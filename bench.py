@@ -1,6 +1,6 @@
 """bench.py -- headline benchmark of the general_cf training hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload simgcl-amazon]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload simgcl-amazon] [--dump-outputs DIR]
 
 One "step" = one iteration of trainer/trainer.py:63-68 (zero_grad, cal_loss, backward, Adam step) at
 B = 4096 on BASELINE.json configs[1]: SimGCL, d = 64, L = 3, tau = 0.2, on a synthetic graph with the
@@ -12,6 +12,9 @@ Prints ONE JSON line (contract in the task statement):
   roofline   the propagation SpMM kernel (HBM-bound): algorithmic bytes / live CUDA-event time
   cpu_baseline  the oracle port of the reference's CPU path, timed on this box's host cores
 ``--impl reference`` times that CPU path alone (rank 0 only under torchrun).
+``--dump-outputs DIR`` writes what the last timed step computed (loss, loss terms, the updated parameters and their
+gradients; a fixed, seeded row sample of arrays too large for the 64 MB budget) as DIR/<name>.npy, so two builds can be compared
+output for output.  It applies to the default GPU arm (not to --impl reference / graph or --workload lightgcn-xl).
 """
 from __future__ import annotations
 
@@ -21,6 +24,7 @@ import math
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -38,7 +42,7 @@ WORKLOADS = {
     'lightgcn-gowalla': ('lightgcn', 'gowalla', dict(layer_num=3, embedding_size=64, reg_weight=1.0e-8, keep_rate=0.5)),
     'sgl-yelp': ('sgl', 'yelp', dict(layer_num=3, embedding_size=64, temperature=0.2, cl_weight=1.0, reg_weight=1.0e-5,
                                      keep_rate=0.5, augmentation='edge_drop')),
-    # BASELINE.json configs[3]: row-sharded over the GPUs (bench_rowshard.py); the whole 10 M x 2 M / 300 M-edge graph at any N
+    # BASELINE.json configs[3]: row-sharded over the GPUs (bench_rowshard.py); the whole 5 M x 1 M / 150 M-edge graph at any N
     'lightgcn-xl': ('lightgcn', 'synthetic-xl', dict(layer_num=3, embedding_size=128, reg_weight=1.0e-8, keep_rate=1.0)),
     'lightgcn-xl-8th': ('lightgcn', 'synthetic-xl-8th', dict(layer_num=3, embedding_size=128, reg_weight=1.0e-8, keep_rate=1.0)),
     'ncl-amazon': ('ncl', 'amazon', dict(layer_num=3, embedding_size=64, high_order=2, reg_weight=1.0e-7, proto_weight=1.0e-4,
@@ -57,7 +61,7 @@ def rank_world():
 
 def graph_arrays(name):
     from synth_graphs import named_graph
-    cache = os.path.join('/tmp', f'sslrec_b200_graph_{name}.npz')
+    cache = os.path.join(tempfile.gettempdir(), f'sslrec_b200_graph_{name}.npz')
     if os.path.exists(cache):
         z = np.load(cache)
         return z['rows'], z['cols'], int(z['n_user']), int(z['n_item'])
@@ -139,12 +143,24 @@ def measured_peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return json.load(open(p)), 'measured'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback (H100 SXM data sheet)'
 
 
 # --------------------------------------------------------------------------------------------------
 # the CPU arm: oracle port of the reference path (oracle/cf_oracle.CpuTrainer)
 # --------------------------------------------------------------------------------------------------
+
+def gpu_identity(index):
+    """Name and power limit of the GPU a number was measured on (both are part of the number)."""
+    out = {'name': torch.cuda.get_device_name(index), 'power_limit_w': None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        out['power_limit_w'] = pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(index)) / 1000.0
+    except Exception as e:      # noqa: BLE001 -- NVML is optional
+        out['power_limit_w'] = 'unavailable: ' + repr(e)[:100]
+    return out
+
 
 def usable_cpus():
     """Host cores this process may actually burn: the affinity mask capped by the cgroup CPU quota (cpu.max)."""
@@ -220,7 +236,7 @@ def run_reference(args):
         print(json.dumps({'impl': 'reference', 'unavailable': f'oracle/_ref is absent and oracle.CpuTrainer has no whole-step driver for {model}'}))
         return
     if graph.startswith('synthetic-xl'):
-        print(json.dumps({'impl': 'reference', 'unavailable': 'config 4 (600 M stored entries) does not fit the bounded CPU sample; see cpu_baseline of lightgcn-xl-8th'}))
+        print(json.dumps({'impl': 'reference', 'unavailable': 'config 4 (300 M stored entries) does not fit the bounded CPU sample; see cpu_baseline of lightgcn-xl-8th'}))
         return
     rows, cols, n_user, n_item = graph_arrays(graph)
     batches = make_batches(rows, cols, n_item, max(2, min(args.steps + args.warmup, 8)))
@@ -315,12 +331,47 @@ def workload_config(name, n_user, n_item, n_edge, world, mode='single'):
             'dim': hp['embedding_size'], 'layers': hp['layer_num'], 'temperature': hp.get('temperature'), 'parallelism': par,
             'propagation': 'one prop_kernel launch per layer and direction (2L per step; a layer needs every row of the previous one), layer sum and '
                            'augmentation fused into the launches',
-            'l2': 'no explicit flush: each step touches > 1 GB (3-view activations, gradient sinks, split partials) >> 126 MB L2'}
+            'l2': 'no explicit flush: each step touches > 1 GB (3-view activations, gradient sinks, split partials) >> 50 MB L2'}
 
 
 # --------------------------------------------------------------------------------------------------
 # the GPU arm
 # --------------------------------------------------------------------------------------------------
+
+DUMP_BYTES = (64 << 20) - (64 << 10)      # all arrays of one dump, .npy headers aside (64 MB in all)
+
+
+def dump_outputs(out_dir, loss, parts, model):
+    """The arrays a caller of the training step receives after it: the loss, every loss term, the updated parameters and
+    their gradients, in float32.  The budget DUMP_BYTES is shared out before anything is written: arrays that fit their
+    share are kept whole, the others keep a sorted row sample drawn with a fixed seed (its row indices are written next
+    to it as <name>.rows.npy, 8 bytes per row counted against the share)."""
+    arrays = {'loss': loss.detach()}
+    arrays.update({'part_' + k: v.detach() for k, v in parts.items()})
+    for name, p in model.named_parameters():
+        arrays['param_' + name] = p.detach()
+        if p.grad is not None:
+            arrays['grad_' + name] = p.grad.detach()
+    arrays = {k: v.float().cpu().numpy() for k, v in arrays.items()}
+    left, order = DUMP_BYTES, sorted(arrays, key=lambda k: arrays[k].nbytes)
+    out = {}
+    for i, name in enumerate(order):                 # smallest first: each takes at most an equal share of what is left
+        a = arrays[name]
+        share = left // (len(order) - i)
+        if a.nbytes > share:
+            row_bytes = a.nbytes // a.shape[0] + 8
+            if share < row_bytes:
+                raise RuntimeError(f'--dump-outputs: one row of {name} does not fit the 64 MB budget')
+            rows = np.sort(np.random.RandomState(0).choice(a.shape[0], size=share // row_bytes, replace=False))
+            out[name + '.rows'] = rows.astype(np.float64)
+            a = a[rows]
+            left -= rows.size * 8
+        out[name] = a
+        left -= a.nbytes
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
 
 def run_ours(args):
     rank, local_rank, world = rank_world()
@@ -378,6 +429,8 @@ def run_ours(args):
         model.kmeans.iters = 20                      # the clustering runs once, before the timed region (ncl.py:73-74)
         model._cluster()
 
+    last_step = {}
+
     def step_resident(i):
         opt.zero_grad()
         b = dev_batches[i % len(dev_batches)]
@@ -386,6 +439,7 @@ def run_ours(args):
         if sync is not None:
             sync.average_gradients(params)
         opt.step()
+        last_step['loss'], last_step['parts'] = loss, parts
         return loss
 
     e2e_sampler = [None]
@@ -473,7 +527,9 @@ def run_ours(args):
     passes = sorted((timed(step_resident, no_sampling=True) for _ in range(5)), key=lambda p: p[0])
     ms_res, launches, _ = passes[2]                      # the MEDIAN pass is the value; all five are in timing_log
     ms_res_best = passes[0][0]
-    ms_res_sampled, _, clocks = timed(step_resident, steps=max(K, 60))      # long enough for several NVML samples
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_step['loss'], last_step['parts'], model)
+    ms_res_sampled, _, clocks = timed(step_resident)
     if clocks is not None:
         clocks['sampled_replay_ms_per_step'] = ms_res_sampled
     # e2e is timed WITHOUT clock sampling (one NVML sample costs ~14 ms of host time, which the per-step
@@ -638,12 +694,12 @@ def run_ours(args):
                     'note': 'achieved / frac / frac_min = compulsory bytes (each input row once, CSR once, epilogue rows) over the live CUDA-event time: '
                             'the HBM roofline; frac_dram = ncu dram bytes of the committed capture over the same time; l2_inclusive_gather_GBps counts a '
                             'gathered row once per stored entry (what the SMs pull through the L2: bounded by the L2 gather rate, not by HBM)'}
-        # the dense InfoNCE contraction (not HBM-bound): on the tcgen05 tensor cores with 3xTF32 error compensation when
+        # the dense InfoNCE contraction (not HBM-bound): on the wgmma tensor cores with 3xTF32 error compensation when
         # dim is 32 / 64, else on the FP32 FMA pipe
         nce = [(m, ms) for name, m, ms in launches_all if name in ('nce_gemm_fwd', 'nce_gemm_bwd')]
         nce_ms = sum(ms for _, ms in nce)
         nce_flops_step = sum(4.0 * m['B'] * m['n'] * m['dim'] for m, _ in nce) / K          # fp32-equivalent: S = R C^T and O += E C
-        sm_mhz = (clocks or {}).get('sm_mhz') or 1965.0
+        sm_mhz = (clocks or {}).get('sm_mhz') or 1980.0
         roofline_nce = None
         if nce:
             used_tc = all(m.get('tc') for m, _ in nce)
@@ -652,14 +708,14 @@ def run_ours(args):
                 peak = peaks['bf16_tflops'] / 2.0
                 roofline_nce = {'kernel': 'softmax_gemm_tc_kernel (ssl_softmax_gemm_tf32x3, forward + backward launches)', 'bound': 'tensor',
                                 'achieved': 3.0 * eq_tf, 'peak': peak, 'unit': 'TFLOP/s', 'frac': 3.0 * eq_tf / peak,
-                                'peak_kind': peak_kind + ' cuBLAS bf16 burst / 2 (kind::tf32 issues at half the bf16 rate)',
+                                'peak_kind': peak_kind + ' bf16 / 2 (tf32 runs at half the bf16 rate)',
                                 'fp32_equivalent_tflops': eq_tf, 'mma_flop_per_step': 3.0 * nce_flops_step,
                                 'note': 'three tf32 products per fp32-grade product (3xTF32)', 'share_of_step': nce_ms / K / prof_ms,
                                 'traffic': ncu_traffic('softmax_gemm_tc_kernel', f'dim{d}_{graph}')}
             else:
-                fp32_peak = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+                fp32_peak = 132 * 128 * 2 * sm_mhz * 1e6 / 1e12
                 roofline_nce = {'kernel': 'softmax_gemm_kernel (ssl_softmax_gemm, forward + backward launches)', 'bound': 'fp32_fma', 'achieved': eq_tf,
-                                'peak': fp32_peak, 'peak_kind': f'148 SM x 128 FMA/clk x 2 x {sm_mhz:.0f} MHz', 'unit': 'TFLOP/s',
+                                'peak': fp32_peak, 'peak_kind': f'132 SM x 128 FMA/clk x 2 x {sm_mhz:.0f} MHz', 'unit': 'TFLOP/s',
                                 'frac': eq_tf / fp32_peak, 'flop_per_step': nce_flops_step, 'share_of_step': nce_ms / K / prof_ms}
         n_prop_layers = max(L, 2 * hp.get('high_order', 0))
         emb_per_step = 2.0 * views * n_prop_layers * nnz if model_name != 'sgl' else 2.0 * L * nnz * (1 + 2 * hp['keep_rate'])
@@ -684,6 +740,7 @@ def run_ours(args):
         value = units * 1e3 / ms_res
         out = {
             'metric': 'train_steps_per_sec', 'value': value, 'unit': 'steps/s', 'n_gpus': world, 'steps': K, 'warmup': W,
+            'gpu': gpu_identity(local_rank),
             'ms_per_step': ms_res, 'higher_is_better': True, 'scaling': scaling_label(args.parallel, args.workload, n_user, n_item, world), 'vs_baseline': None, 'dtype': 'f32',
             'data': 'synthetic', 'config': workload_config(args.workload, n_user, n_item, len(rows), world, mode),
             'batches_per_sync_step': units, 'optimizer_steps_per_sec': 1e3 / ms_res,
@@ -811,7 +868,7 @@ def run_graph(args):
 
 
 def run_xl(args):
-    """BASELINE.json configs[3]: LightGCN on the synthetic 10 M x 2 M / 300 M-edge graph, d = 128, row-sharded over the
+    """BASELINE.json configs[3]: LightGCN on the synthetic 5 M x 1 M / 150 M-edge graph, d = 128, row-sharded over the
     GPUs (strong scaling: the same graph at every N).  The bench line's value is the sharded step; rank 0's single-GPU run
     of the same graph is measured in the same process when N > 1 (``row_shard.baselines``)."""
     rank, local_rank, world = rank_world()
@@ -835,6 +892,8 @@ def run_xl(args):
             sampler.sample()
         peaks, peak_kind = measured_peaks()
         one = rec if world > 1 else rec['baselines']['one_gpu_config4']
+        if 'ms_per_step' not in one:
+            raise SystemExit(f'bench.py: the config-4 step did not run: {one.get("error")}')
         ms, spmm_ms, n_launch = one['ms_per_step'], one['spmm_ms'], max(1.0, one.get('spmm_launches', 2 * R.LAYERS))
         n_user, n_item, n_edge = R.EIGHTH[0] * 8, R.EIGHTH[1] * 8, R.EIGHTH[2] * 8
         nnz_rank = one.get('nnz_per_rank', one.get('nnz'))
@@ -853,7 +912,7 @@ def run_xl(args):
             'config': {'workload': 'lightgcn training step on the synthetic config-4 graph (BASELINE.json configs[3])', 'model_name': 'lightgcn', 'graph': 'synthetic-xl',
                        'n_user': n_user, 'n_item': n_item, 'nnz': 2 * n_edge, 'batch': BATCH, 'global_batch': BATCH, 'dim': R.DIM, 'layers': R.LAYERS,
                        'parallelism': ('single GPU' if world == 1 else f'x{world}: rows of A and E sharded, all-gather of every layer output fused into the SpMM epilogue (NVLink peer stores)'),
-                       'l2': 'no explicit flush: the 6.1 GB tables exceed the 126 MB L2 by 50x'},
+                       'l2': 'no explicit flush: the 3.1 GB tables exceed the 50 MB L2 by 60x'},
             'e2e': {'value': 1e3 / one['e2e_ms_per_step'], 'unit': 'steps/s', 'ms_per_step': one['e2e_ms_per_step'], 'h2d_bytes_per_step': 3 * BATCH * 8, 'd2h_bytes_per_step': 4,
                     'how': 'batch from pinned host memory -> H2D, cal_loss, backward, (sharded) FusedAdam.step, loss.item() every step'},
             'gpu_launches': launches,
@@ -881,6 +940,7 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference', 'graph'])
     ap.add_argument('--workload', default='simgcl-amazon', choices=sorted(WORKLOADS))
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed step as DIR/<name>.npy')
     ap.add_argument('--no-cuda-graph', action='store_true', help='skip the cuda_graph record (e.g. under a profiler)')
     ap.add_argument('--no-eval-kernels', action='store_true', help='skip the eval_kernels record (predict / top-k / k-means timings in a subprocess)')
     ap.add_argument('--cpu-budget', type=float, default=170.0, help='--impl reference: wall-clock budget of the timed CPU steps (s)')
@@ -892,6 +952,8 @@ def main():
                     help='N > 1: dp = one batch per GPU + gradient all-reduce (weak scaling); shard = one batch, table rows sharded')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
+    if args.dump_outputs and (args.impl != 'ours' or args.workload == 'lightgcn-xl'):
+        ap.error('--dump-outputs applies to the default GPU arm only (not to --impl reference / graph or --workload lightgcn-xl)')
     if args.impl == 'reference':
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
-"""Row-sharded LightGCN training step on the BASELINE.json config-4 graph family (10 M x 2 M nodes, 300 M edges, d = 128,
-L = 3), used by bench.py: north_star's multi-GPU partition -- adjacency rows and the embedding table row-sharded over
+"""Row-sharded LightGCN training step on the BASELINE.json config-4 graph family (5 M x 1 M nodes, 150 M edges, d = 128,
+L = 3: the whole graph trains on one 80 GB H100), used by bench.py: north_star's multi-GPU partition -- adjacency rows and the embedding table row-sharded over
 the GPUs, the all-gather of each layer output fused into the SpMM epilogue as NVLink peer stores (sslrec_b200/parallel.py).
 
 ``leg(...)`` measures, on ``world`` GPUs, the graph scaled to world/8 of config 4 (per-GPU work fixed: weak scaling) and
@@ -18,12 +18,12 @@ import synth_graphs as S
 
 BATCH = 4096
 DIM, LAYERS = 128, 3
-EIGHTH = (1_250_000, 250_000, 37_500_000)          # |U|, |I|, E of one eighth of config 4
+EIGHTH = (625_000, 125_000, 18_750_000)            # |U|, |I|, E of one eighth of config 4
 
 
 class DeviceGraphHandler:
     """The attributes a general_cf model reads from its data handler, for a graph that only exists as device arrays:
-    no torch sparse COO tensor is ever built (config 4 has 600 M stored entries); ``plan_source`` hands the model the CSR
+    no torch sparse COO tensor is ever built (config 4 has 300 M stored entries); ``plan_source`` hands the model the CSR
     of the row ranges it owns."""
 
     def __init__(self, keys: torch.Tensor, n_user: int, n_item: int):
@@ -131,15 +131,18 @@ def _time_steps(model, opt, batches, steps, warmup, dist, dev):
 
 
 def _single_gpu(keys, n_user, n_item, dev, steps, warmup):
+    torch.cuda.reset_peak_memory_stats(dev)
     model, opt, handler = _build(keys, n_user, n_item, dev, None)
     batches = _make_batches(keys, n_item, steps + warmup, dev, 7)
     ms, summ, loss = _time_steps(model, opt, batches, steps, warmup, None, dev)
     stats = handler.last_plan.stats()
     nnz = handler.last_plan.nnz
+    peak_gb = torch.cuda.max_memory_allocated(dev) / 1e9
     del model, opt, handler, batches
     torch.cuda.empty_cache()
     return dict(ms_per_step=ms, e2e_ms_per_step=summ['e2e_ms_per_step'], spmm_ms=summ.get('prop_fwd', {}).get('ms', 0.0) + summ.get('prop_bwd', {}).get('ms', 0.0),
-                spmm_launches=summ.get('prop_fwd', {}).get('launches', 0) + summ.get('prop_bwd', {}).get('launches', 0), nnz=nnz, max_row_nnz=stats['max_row_nnz'], loss=loss, first_loss=summ['first_loss'])
+                spmm_launches=summ.get('prop_fwd', {}).get('launches', 0) + summ.get('prop_bwd', {}).get('launches', 0), nnz=nnz, max_row_nnz=stats['max_row_nnz'], loss=loss, first_loss=summ['first_loss'],
+                peak_mem_gb=peak_gb)
 
 
 def leg(dist, rank, world, dev, steps=5, warmup=2, full=False, baselines=True, log=lambda *a: None):
@@ -148,7 +151,7 @@ def leg(dist, rank, world, dev, steps=5, warmup=2, full=False, baselines=True, l
     scale = 8 if full else world
     n_user, n_item, n_edge = (EIGHTH[0] * scale, EIGHTH[1] * scale, EIGHTH[2] * scale)
     t0 = time.perf_counter()
-    # rank 0 generates, everyone receives the same sorted unique edge keys (2.4 GB at config 4: milliseconds over NVLink)
+    # rank 0 generates, everyone receives the same sorted unique edge keys (1.2 GB at config 4: milliseconds over NVLink)
     if rank == 0:
         keys = S.bipartite_keys_device(n_user, n_item, n_edge, 2023, 1.0, dev)
     else:
@@ -196,7 +199,7 @@ def leg(dist, rank, world, dev, steps=5, warmup=2, full=False, baselines=True, l
                     'loss': loss, 'first_loss': summ['first_loss'], 'steps': steps, 'warmup': warmup})
         rec['multicast'] = bool(comm._tables and next(iter(comm._tables.values())).mc_ptr)
         del model, opt, handler, batches
-        comm._tables.clear()                                  # the shared tables (6.1 GB each at config 4) go before rank 0's one-GPU baselines
+        comm._tables.clear()                                  # the shared tables (3.1 GB each at config 4) go before rank 0's one-GPU baselines
         comm._barrier_handle = None
         del comm
         import gc

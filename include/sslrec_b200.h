@@ -1,5 +1,5 @@
 /*
- * sslrec_b200 -- C ABI of the B200 (sm_100a) general_cf training hot path.
+ * sslrec_b200 -- C ABI of the H100 (sm_90a) general_cf training hot path.
  *
  * The reference (HKUDS/SSLRec) has no FFI: its "operator interface" for this path is the set of
  * PyTorch calls made by models/general_cf/*.py, models/loss_utils.py, models/aug_utils.py and
@@ -52,7 +52,7 @@ SSL_API const char *ssl_last_error(void);
 SSL_API int64_t ssl_launch_count(void);
 /* process-wide switches for tests and A/B profiling (value 0 / 1):
  *   "prop_view_major"  propagation with grid.y = view and one accumulator per thread: DRAM traffic at 1.03x compulsory instead of
- *                      1.3x, but 25-40 % slower on B200 (profiles/r02_prop_variants.md); default 0
+ *                      1.3x, at the cost of less work per thread (the kernel is issue / latency bound); default 0
  *   "kmeans_rows_per_round"  1 selects kmeans_assign_kernel<1> (one row per warp and round, the round-1 form); default 4 rows per round --
  *                      same arithmetic per (row, centroid), same summation order: bit-identical results (csrc/kmeans_assign.cuh)
  *   "predict_tiled"    ssl_predict_mask as a register-tiled product (128 x 128 score tiles, csrc/predict_tile.cuh); 0 selects the
@@ -221,7 +221,7 @@ SSL_API int ssl_rows_normalize(const float *x, int64_t stride, const int64_t *id
 SSL_API int ssl_softmax_gemm(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int32_t dim,
                      const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                      void *stream);
-/* The same contraction on the tcgen05 tensor cores with 3xTF32 error compensation (fp32-grade
+/* The same contraction on the Hopper tensor cores (wgmma) with 3xTF32 error compensation (fp32-grade
  * accuracy): operands are the hi / lo splits written by ssl_rows_normalize, row-major [n, dim],
  * and for the streamed operand also the transposed splits CT_hi / CT_lo [dim, ct_pitch];
  * dim must be 32 or 64.  colscale, when given, must be readable up to ceil64(n_c) floats (the

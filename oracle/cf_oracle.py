@@ -14,7 +14,7 @@ reference and the CUDA path can be driven by the same bits.
 
 Parity pinning: the reference ships no tests or golden vectors for this path
 (SURVEY.md section 4), so the oracle is pinned against the reference itself:
-``oracle/gen_golden.py`` imports the unmodified reference from ``/root/reference``,
+``oracle/gen_golden.py`` imports the unmodified reference from ``$SSLREC_REFERENCE``,
 runs it on injected inputs and writes ``tests/golden/*.npz``; ``tests/test_oracle_golden.py``
 checks this module against those files.
 """

@@ -1,8 +1,7 @@
-"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference (HKUDS/SSLRec at
-/root/reference) on CPU with injected inputs.  TEST INFRASTRUCTURE ONLY.
+"""Generate ``tests/golden/*.npz`` by running the UNMODIFIED reference (HKUDS/SSLRec, the
+checkout named by $SSLREC_REFERENCE) on CPU with injected inputs.  TEST INFRASTRUCTURE ONLY.
 
-Runs only in the build container (needs /root/reference); the outputs are committed so
-the GPU box never needs the reference.  Usage:
+Needs the reference checkout; the outputs are committed so the tests never need the reference.  Usage:
 
     python oracle/gen_golden.py            # all cases (one subprocess per case)
     python oracle/gen_golden.py --one lightgcn tiny
@@ -30,7 +29,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = '/root/reference'
+REF = os.environ.get('SSLREC_REFERENCE', '/root/reference')
 OUT = os.path.join(ROOT, 'tests', 'golden')
 
 # model -> overrides of configs['model'] (BASELINE.json values where they differ from the YAML)

@@ -71,7 +71,7 @@ class BaseModel(nn.Module):
         self._inject = None        # tests: dict of injected masks / noise
         self.comm = None           # parallel.RowShard for row-sharded multi-GPU runs
         # optional: data_handler.plan_source(device, row_ranges, side_split) -> GraphPlan builds the CSR plan without a
-        # torch sparse COO tensor (BASELINE config 4: 600 M stored entries are generated and sorted on the device)
+        # torch sparse COO tensor (BASELINE config 4: 300 M stored entries are generated and sorted on the device)
         self._plan_source = getattr(data_handler, 'plan_source', None)
 
     def _plan(self, adj=None) -> GraphPlan:

@@ -1,4 +1,4 @@
-// Shared helpers for the sslrec_b200 kernels (sm_100a).
+// Shared helpers for the sslrec_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -40,7 +40,7 @@ extern int g_predict_tiled;   // ssl_set_option("predict_tiled", v): 1 (default)
         ssl::count_launch();                                                                   \
     } while (0)
 
-constexpr int kNumSM = 148;   // B200
+constexpr int kNumSM = 132;   // H100 SXM
 
 // ---------------------------------------------------------------------------------------------
 // Philox4x32-10 counter-based RNG.  One call -> 4 x 32 random bits, keyed by a 64-bit seed and a

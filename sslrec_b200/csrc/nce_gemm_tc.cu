@@ -1,5 +1,5 @@
-// ssl_softmax_gemm_tf32x3: the InfoNCE contraction on the 5th-generation tensor cores (tcgen05,
-// kind::tf32) with fp32-grade accuracy through 3xTF32 error compensation.
+// ssl_softmax_gemm_tf32x3: the InfoNCE contraction on the Hopper tensor cores (wgmma, tf32) with
+// fp32-grade accuracy through 3xTF32 error compensation.
 //
 //   S  = R C^T   = R_hi C_hi^T + R_lo C_hi^T + R_hi C_lo^T          (x = x_hi + x_lo, x_hi = tf32(x))
 //   E  = exp2(S - offset) * colscale ;  rowsum += sum_c E
@@ -10,28 +10,20 @@
 // dropped lo*lo products and the rounding of the lo parts are O(2^-22) relative and unbiased -- the fp32
 // rounding level of the FFMA kernel.
 //
-// Structure (one CTA per SM, 256 threads, warp-specialised, all synchronisation by mbarriers):
-//   warp 0 / lane 0 : TMA producer, ring 1.  2-D tensor maps (SWIZZLE_128B, 32-float boxes) over the
-//                     row-major hi / lo operand arrays: the resident 128-row R tile once, then the 64-row
-//                     C tiles (GEMM1's B operand, K-major; freed as soon as GEMM1 of the tile retires).
-//   warp 2 / lane 0 : TMA producer, ring 2: the same tiles from the TRANSPOSED copies [d, n] (GEMM2's B
-//                     operand, K-major again).  tf32 operands must be K-major here: an MN-major view of
-//                     the row-major tile needs the 32-byte-atom swizzle, which the K-major GEMM1 view of
-//                     the same bytes cannot share (measured: the MN-major descriptor yields zeros).
-//   warp 1 / lane 0 : MMA issuer 1.  GEMM1 (M=128, N=64, K=d): both operands in shared memory -> S in TMEM.
-//   warp 3 / lane 0 : MMA issuer 2.  GEMM2 (M=128, N=d, K=64): A = E read from TENSOR MEMORY, B = C^T tile ->
-//                     O in TMEM, accumulated over all tiles.  Two issuing threads because tf32 MMAs are only
-//                     K = 8 deep: one thread cannot issue them as fast as the tensor pipe retires them.
-//   warps 4-11,12-19: two epilogue groups (256 threads each) ping-ponging over the tiles (parity); thread =
-//                     (TMEM lane = row, one 32-column half of the tile).  tcgen05.ld S (which frees the S
-//                     buffer for the next GEMM1 at once), ex2, row sums in registers, tf32 split of E,
-//                     tcgen05.st E_hi / E_lo into their own TMEM buffers; finally O is read out once per CTA.
-//   Roofline: 65536 MACs per K=8 MMA at the measured tf32 peak (cuBLAS bf16 burst / 2 = 865 TFLOP/s) is ~44 SM cycles,
-//   48 MMAs per 64-column tile = ~2100 cycles; measured 2350 cycles per tile at the bench's forward shape
-//   (0.339 ms, 777 TFLOP/s of tf32 MMA work = 90 % of that peak).  Tried and dropped: the resident operand's
-//   hi part in TMEM (TS-form GEMM1, single S buffer) -- same speed, slower backward shape.
-//   TMEM columns    : [0,128) S x2, [128,256) E_hi x2, [256,384) E_lo x2, [384,384+d) O (hi*hi),
-//                     [448,448+d) O correction terms -- all 512 columns.
+// Structure (one CTA per SM, 384 threads = 3 warpgroups, all synchronisation by mbarriers):
+//   warpgroup 0, one thread : TMA producer.  2-D tensor maps (SWIZZLE_128B, 32-float boxes) over the row-major
+//                     hi / lo operand arrays: the resident 128-row R tile once, then per 64-row C tile one ring
+//                     stage holding the row-major C tile (GEMM1's B operand) and the tile of the TRANSPOSED copy
+//                     [d, n] (GEMM2's B operand).  wgmma reads tf32 operands from shared memory K-major only,
+//                     which is why both copies are streamed.
+//   warpgroups 1, 2 : consumers, 64 rows of the R tile each, over all C tiles of the CTA:
+//                     GEMM1 (m64 n64 k8, both operands in shared memory) -> S in registers;  E = exp2(S - offset)
+//                     with the row sums in registers;  the accumulator fragment of S is permuted by warp shuffles
+//                     into the A-operand fragment of GEMM2 and split into tf32 hi / lo there;  GEMM2 (m64 nD k8,
+//                     A = E from registers, B = C^T tile) accumulates O.  The two warpgroups interleave their exp
+//                     phases with each other's MMAs.
+//   The two correction products of GEMM2 go to their own accumulator: the tensor core does not round its fp32
+//   accumulations to nearest, so the long hi*hi sum must not also carry them.
 #include <cuda.h>
 #include <cstdlib>
 
@@ -40,10 +32,17 @@
 namespace {
 
 constexpr int BM = 128, BN = 64;
-constexpr int ST1 = 3, ST2 = 2;        // stages of ring 1 (GEMM1's B, gates the S pipeline) and ring 2 (GEMM2's B); 64 + 96 + 64 KB at d = 64
-constexpr int kNumThreads = 640;       // warps 0-3: TMA, MMA1, TMA, MMA2; warps 4-11 and 12-19: two epilogue groups of 256 threads
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t COL_S = 0, COL_EHI = 128, COL_ELO = 256, COL_O = 384, COL_OC = 448;
+constexpr int kNumThreads = 384;       // warpgroup 0: TMA producer; warpgroups 1, 2: consumers (64 rows each)
+
+template <int D> struct Cfg {
+    static constexpr int KCH = D / 32;                  // 128-byte K chunks per operand row (GEMM1: K = d)
+    static constexpr int JCH = BN / 32;                 // 128-byte K chunks of the transposed tile (GEMM2: K = 64 rows)
+    static constexpr uint32_t R_CHUNK = BM * 128, C_CHUNK = BN * 128, T_CHUNK = D * 128;
+    static constexpr uint32_t R_BYTES = KCH * R_CHUNK, C_BYTES = KCH * C_CHUNK, T_BYTES = JCH * T_CHUNK;   // one precision part
+    static constexpr uint32_t STAGE_BYTES = 2 * C_BYTES + 2 * T_BYTES;
+    static constexpr int ST = (D == 32) ? 4 : 2;        // ring stages: 64 KB R + 2 x 64 KB at d = 64, 32 KB R + 4 x 32 KB at d = 32
+    static constexpr size_t SMEM = 1024 + 2 * (size_t)R_BYTES + (size_t)ST * STAGE_BYTES + (2 * ST + 1) * sizeof(uint64_t);
+};
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -71,139 +70,116 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-// exactly one lane of a fully converged warp (warp-uniform control flow around it keeps the operands of
-// the MMA / commit instructions in uniform registers: no per-lane "waterfall" loop around every UTCHMMA)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "elect.sync _|p, 0xffffffff;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Four consecutive K-steps (one 128-byte swizzle chunk = 32 tf32) in ONE asm block: the descriptors advance by
-// 32 bytes (+2 in the 16-byte-unit address field) inside the block, so the single issuing thread spends ~3
-// instructions per MMA instead of ~15 (ncu round 1: the contraction was bound by the MMA issue loop, not by the
-// tensor pipe).  acc_first: whether the first of the four accumulates onto D; the other three always do.
-__device__ __forceinline__ void mma_ss_x4(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc_first) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p, t;\n"
-        ".reg .b64 a, b;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "setp.eq.b32 t, 0, 0;\n"
-        "mov.b64 a, %1;\n"
-        "mov.b64 b, %2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], a, b, %3, p;\n"
-        "add.s64 a, a, 2;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], a, b, %3, t;\n"
-        "add.s64 a, a, 2;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], a, b, %3, t;\n"
-        "add.s64 a, a, 2;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], a, b, %3, t;\n"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc_first) : "memory");
-}
-__device__ __forceinline__ void mma_ts_x4(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t acc_first) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p, t;\n"
-        ".reg .b64 b;\n"
-        ".reg .b32 a;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "setp.eq.b32 t, 0, 0;\n"
-        "mov.b32 a, %1;\n"
-        "mov.b64 b, %2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [a], b, %3, p;\n"
-        "add.s32 a, a, 8;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [a], b, %3, t;\n"
-        "add.s32 a, a, 8;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [a], b, %3, t;\n"
-        "add.s32 a, a, 8;\n add.s64 b, b, 2;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [a], b, %3, t;\n"
-        "}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(acc_first) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-          "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-          "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-          "r"(v[30]), "r"(v[31])
-        : "memory");
-}
 __device__ __forceinline__ float ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): SWIZZLE_128B, version 1
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
+// ---- wgmma (sm_90a) ----
+// shared-memory matrix descriptor: K-major, SWIZZLE_128B (layout type 1), 8-row core-matrix groups 1024 bytes apart.
+// A K step of 8 tf32 inside the 128-byte swizzle atom advances the start address by 32 bytes.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t addr) {
+    return (uint64_t)((addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = f32, A = B = tf32
-__host__ __device__ constexpr uint32_t instr_desc(int m, int n, int b_mn_major) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps registers an asynchronous wgmma reads or writes live (and in place) up to this point
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void reg_fence(uint32_t (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
-// one 32-column chunk of a tile: S -> E, row sum, tf32 split
+// d[64 x 64] (+)= A[smem] * B[smem]^T
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc));
+}
+// d[64 x 64] += A[registers, one k8 block] * B[smem]^T
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t *a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1;\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+// d[64 x 32] += A[registers, one k8 block] * B[smem]^T
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t *a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1;\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+template <int D>
+__device__ __forceinline__ void wgmma_rs(float (&d)[D / 2], const uint32_t *a, uint64_t b) {
+    if constexpr (D == 64) wgmma_rs_n64(d, a, b);
+    else wgmma_rs_n32(d, a, b);
+}
+
+// One 64-column tile of S (accumulator fragment: s[4j + 2h + c] = S(row g + 8h, col 8j + 2t + c), g = lane / 4,
+// t = lane % 4) -> E, the two row sums, and E as GEMM2's A fragment in tf32 hi / lo: a[4j + h] = E(g + 8h, 8j + t),
+// a[4j + 2 + h] = E(g + 8h, 8j + t + 4).  The column permutation is a shuffle among the four lanes of a row group.
 template <bool CHECK>
-__device__ __forceinline__ void exp_chunk(uint32_t (&v)[32], uint32_t (&lo)[32], float offset, const float *__restrict__ cs_ptr,
-                                          int64_t col, int64_t n_c, float &rowsum) {
+__device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[32], uint32_t (&alo)[32], float offset,
+                                         const float *__restrict__ cs_ptr, int64_t col0, int64_t n_c, float (&rowsum)[2]) {
+    const int lane = threadIdx.x & 31, t = lane & 3;
+    const int src1 = (lane & ~3) | (t >> 1), src2 = src1 + 2;
+    const bool odd = (t & 1) != 0;
 #pragma unroll
-    for (int k = 0; k < 32; k += 4) {
-        float cs[4] = {1.f, 1.f, 1.f, 1.f};
+    for (int j = 0; j < 8; ++j) {
+        const int64_t col = col0 + 8 * j + 2 * t;
+        float cs0 = 1.f, cs1 = 1.f;
         if (cs_ptr != nullptr) {
-            const float4 c4 = __ldg(reinterpret_cast<const float4 *>(cs_ptr + col + k));
-            cs[0] = c4.x; cs[1] = c4.y; cs[2] = c4.z; cs[3] = c4.w;
+            if (!CHECK) {
+                const float2 c2 = __ldg(reinterpret_cast<const float2 *>(cs_ptr + col));
+                cs0 = c2.x; cs1 = c2.y;
+            } else {
+                cs0 = col < n_c ? __ldg(cs_ptr + col) : 0.f;
+                cs1 = col + 1 < n_c ? __ldg(cs_ptr + col + 1) : 0.f;
+            }
         }
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            float e = ex2(__uint_as_float(v[k + u]) - offset) * cs[u];
-            if (CHECK) e = (col + k + u < n_c) ? e : 0.f;
-            rowsum += e;
-            float ehi, elo;
-            ssl::tf32_split(e, ehi, elo);
-            v[k + u] = __float_as_uint(ehi);
-            lo[k + u] = __float_as_uint(elo);
+        for (int h = 0; h < 2; ++h) {
+            float e0 = ex2(s[4 * j + 2 * h] - offset) * cs0;
+            float e1 = ex2(s[4 * j + 2 * h + 1] - offset) * cs1;
+            if (CHECK) {
+                e0 = (col < n_c) ? e0 : 0.f;
+                e1 = (col + 1 < n_c) ? e1 : 0.f;
+            }
+            rowsum[h] += e0 + e1;
+            const float v0 = __shfl_sync(0xffffffffu, e0, src1), v1 = __shfl_sync(0xffffffffu, e1, src1);
+            const float w0 = __shfl_sync(0xffffffffu, e0, src2), w1 = __shfl_sync(0xffffffffu, e1, src2);
+            float hi, lo;
+            ssl::tf32_split(odd ? v1 : v0, hi, lo);
+            ahi[4 * j + h] = __float_as_uint(hi);
+            alo[4 * j + h] = __float_as_uint(lo);
+            ssl::tf32_split(odd ? w1 : w0, hi, lo);
+            ahi[4 * j + 2 + h] = __float_as_uint(hi);
+            alo[4 * j + 2 + h] = __float_as_uint(lo);
         }
     }
 }
@@ -215,22 +191,16 @@ softmax_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_r_hi, const __gri
                        const __grid_constant__ CUtensorMap map_ct_hi, const __grid_constant__ CUtensorMap map_ct_lo,
                        int64_t n_r, int64_t n_c, const float *__restrict__ colscale, float offset, int n_split,
                        float *__restrict__ rowsum_part, float *__restrict__ o_part) {
-    constexpr int KCH = D / 32;                         // 128-byte K chunks per operand row (GEMM1: K = d)
-    constexpr int JCH = BN / 32;                        // 128-byte K chunks of the transposed tile (GEMM2: K = 64 rows)
-    constexpr uint32_t R_CHUNK = BM * 128, C_CHUNK = BN * 128, T_CHUNK = D * 128;
-    constexpr uint32_t R_BYTES = KCH * R_CHUNK, C_BYTES = KCH * C_CHUNK, T_BYTES = JCH * T_CHUNK;   // one precision part
+    using K = Cfg<D>;
+    constexpr int ST = K::ST, KCH = K::KCH, JCH = K::JCH;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *r_hi = smem, *r_lo = smem + R_BYTES;
-    uint8_t *ring1 = smem + 2 * R_BYTES;                // stage s: C tile row-major, hi then lo (GEMM1's B, K-major)
-    uint8_t *ring2 = ring1 + ST1 * 2 * C_BYTES;      // stage s: C^T tile, hi then lo          (GEMM2's B, K-major)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(ring2 + ST2 * 2 * T_BYTES);
-    uint64_t *full1 = bars, *empty1 = full1 + ST1, *full2 = empty1 + ST1, *empty2 = full2 + ST2;
-    uint64_t *s_full = empty2 + ST2, *s_free = s_full + 2, *e_ready = s_free + 2, *e_free = e_ready + 2, *r_full = e_free + 2, *o_full = r_full + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(o_full + 1);
-    float *rowsum_x = reinterpret_cast<float *>(tmem_slot + 4);     // [3][128] partial row sums of the other epilogue sub-groups
+    uint8_t *r_hi = smem, *r_lo = smem + K::R_BYTES;
+    uint8_t *ring = smem + 2 * K::R_BYTES;               // stage s: C hi, C lo (row-major tile), C^T hi, C^T lo
+    uint64_t *full = reinterpret_cast<uint64_t *>(ring + ST * K::STAGE_BYTES);
+    uint64_t *empty = full + ST, *r_full = empty + ST;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
     const int rt = blockIdx.x / n_split, sp = blockIdx.x % n_split;
     const int64_t n_ct = (n_c + BN - 1) / BN;
     const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
@@ -244,184 +214,121 @@ softmax_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_r_hi, const __gri
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_lo));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ct_hi));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ct_lo));
-        for (int s = 0; s < ST1; ++s) {
-            mbar_init(&full1[s], 1);
-            mbar_init(&empty1[s], 1);
-        }
-        for (int s = 0; s < ST2; ++s) {
-            mbar_init(&full2[s], 1);
-            mbar_init(&empty2[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&s_full[b], 1);
-            mbar_init(&s_free[b], 256);
-            mbar_init(&e_ready[b], 256);
-            mbar_init(&e_free[b], 1);
+        for (int s = 0; s < ST; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 256);
         }
         mbar_init(r_full, 1);
-        mbar_init(o_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0 && lane == 0) {
-        // ===================== TMA producer, ring 1: R tile once, then the row-major C tiles =====================
-        mbar_expect_tx(r_full, 2 * R_BYTES);
-        for (int c = 0; c < KCH; ++c) {
-            tma_load_2d(r_hi + c * R_CHUNK, &map_r_hi, c * 32, row0, r_full);
-            tma_load_2d(r_lo + c * R_CHUNK, &map_r_lo, c * 32, row0, r_full);
-        }
-        for (int i = 0; i < n_tiles; ++i) {
-            const int s = i % ST1;
-            mbar_wait(&empty1[s], ((i / ST1) & 1) ^ 1);
-            uint8_t *hi = ring1 + s * 2 * C_BYTES, *lo = hi + C_BYTES;
-            mbar_expect_tx(&full1[s], 2 * C_BYTES);
+    if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+        if (threadIdx.x == 0) {
+            // ===================== TMA producer: R tile once, then per C tile its row-major and transposed copies =====================
+            mbar_expect_tx(r_full, 2 * K::R_BYTES);
             for (int c = 0; c < KCH; ++c) {
-                tma_load_2d(hi + c * C_CHUNK, &map_c_hi, c * 32, (t0 + i) * BN, &full1[s]);
-                tma_load_2d(lo + c * C_CHUNK, &map_c_lo, c * 32, (t0 + i) * BN, &full1[s]);
+                tma_load_2d(r_hi + c * K::R_CHUNK, &map_r_hi, c * 32, row0, r_full);
+                tma_load_2d(r_lo + c * K::R_CHUNK, &map_r_lo, c * 32, row0, r_full);
             }
-        }
-    } else if (warp == 2 && lane == 0) {
-        // ===================== TMA producer, ring 2: the transposed C tiles [d, 64] =====================
-        for (int i = 0; i < n_tiles; ++i) {
-            const int s = i % ST2;
-            mbar_wait(&empty2[s], ((i / ST2) & 1) ^ 1);
-            uint8_t *hi = ring2 + s * 2 * T_BYTES, *lo = hi + T_BYTES;
-            mbar_expect_tx(&full2[s], 2 * T_BYTES);
-            for (int c = 0; c < JCH; ++c) {
-                tma_load_2d(hi + c * T_CHUNK, &map_ct_hi, (t0 + i) * BN + c * 32, 0, &full2[s]);
-                tma_load_2d(lo + c * T_CHUNK, &map_ct_lo, (t0 + i) * BN + c * 32, 0, &full2[s]);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer 1: S = R C^T (three tf32 products, small ones first) =====================
-        constexpr uint32_t idesc1 = instr_desc(BM, BN, 0);      // S[128 x 64] = R (K-major, K = d) x C (K-major)
-        const uint32_t r_hi_a = smem_u32(r_hi), r_lo_a = smem_u32(r_lo);
-        mbar_wait(r_full, 0);
-        for (int i = 0; i < n_tiles; ++i) {
-            const int s = i % ST1, b = i & 1;
-            mbar_wait(&full1[s], (i / ST1) & 1);
-            mbar_wait(&s_free[b], ((i >> 1) & 1) ^ 1);           // the epilogue of tile i-2 has read S out of this buffer
-            tc_fence_after();
-            const uint32_t c_hi_a = smem_u32(ring1 + s * 2 * C_BYTES), c_lo_a = c_hi_a + C_BYTES;
-#pragma unroll
-            for (int part = 0; part < 3; ++part) {
-                const uint32_t ra = (part == 0) ? r_lo_a : r_hi_a;
-                const uint32_t cb = (part == 1) ? c_lo_a : c_hi_a;
-#pragma unroll
-                for (int c = 0; c < KCH; ++c)
-                    if (elect_one())
-                        mma_ss_x4(tmem + COL_S + b * BN, smem_desc(ra + c * R_CHUNK, 16, 1024), smem_desc(cb + c * C_CHUNK, 16, 1024), idesc1,
-                                  (part > 0 || c > 0) ? 1u : 0u);
-            }
-            if (elect_one()) {
-                tc_commit(&s_full[b]);
-                tc_commit(&empty1[s]);                          // GEMM1 was the only reader of this stage
-            }
-            __syncwarp();
-        }
-    } else if (warp == 3) {
-        // ===================== MMA issuer 2: O += E C  (A = E from TMEM, B = C^T tile) =====================
-        constexpr uint32_t idesc2 = instr_desc(BM, D, 0);       // O[128 x d] += E (TMEM, K = 64) x C^T (K-major)
-        for (int j = 0; j < n_tiles; ++j) {
-            const int s = j % ST2, b = j & 1;
-            mbar_wait(&e_ready[b], (j >> 1) & 1);
-            mbar_wait(&full2[s], (j / ST2) & 1);
-            tc_fence_after();
-            const uint32_t t_hi_a = smem_u32(ring2 + s * 2 * T_BYTES), t_lo_a = t_hi_a + T_BYTES;
-            const uint32_t e_hi = tmem + COL_EHI + b * BN, e_lo = tmem + COL_ELO + b * BN;
-            // the two correction products go to their own accumulator: the tensor core rounds its fp32
-            // accumulations toward zero, so the long hi*hi sum must not also carry them
-#pragma unroll
-            for (int part = 0; part < 3; ++part) {
-                const uint32_t ea = (part == 0) ? e_lo : e_hi;
-                const uint32_t tb = (part == 1) ? t_lo_a : t_hi_a;
-                const uint32_t od = tmem + ((part == 2) ? COL_O : COL_OC);
-#pragma unroll
+            for (int i = 0; i < n_tiles; ++i) {
+                const int s = i % ST;
+                mbar_wait(&empty[s], ((i / ST) & 1) ^ 1);
+                uint8_t *c_hi = ring + s * K::STAGE_BYTES, *c_lo = c_hi + K::C_BYTES;
+                uint8_t *ct_hi = c_lo + K::C_BYTES, *ct_lo = ct_hi + K::T_BYTES;
+                mbar_expect_tx(&full[s], K::STAGE_BYTES);
+                for (int c = 0; c < KCH; ++c) {
+                    tma_load_2d(c_hi + c * K::C_CHUNK, &map_c_hi, c * 32, (t0 + i) * BN, &full[s]);
+                    tma_load_2d(c_lo + c * K::C_CHUNK, &map_c_lo, c * 32, (t0 + i) * BN, &full[s]);
+                }
                 for (int c = 0; c < JCH; ++c) {
-                    const bool first = (part == 2) ? (c == 0) : (part == 0 && c == 0);
-                    if (elect_one()) mma_ts_x4(od, ea + c * 32, smem_desc(tb + c * T_CHUNK, 16, 1024), idesc2, (j > 0 || !first) ? 1u : 0u);
+                    tma_load_2d(ct_hi + c * K::T_CHUNK, &map_ct_hi, (t0 + i) * BN + c * 32, 0, &full[s]);
+                    tma_load_2d(ct_lo + c * K::T_CHUNK, &map_ct_lo, (t0 + i) * BN + c * 32, 0, &full[s]);
                 }
             }
-            if (elect_one()) {
-                tc_commit(&empty2[s]);
-                tc_commit(&e_free[b]);
-            }
-            __syncwarp();
         }
-        if (elect_one()) tc_commit(o_full);
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ===== epilogue: two groups of 8 warps ping-pong over the tiles (group g owns the tiles and TMEM buffers of
-        // ===== parity g); inside a group, thread = (TMEM lane = row, one 32-column half of the 64-column tile)
-        const int e = warp - 4;
-        const int g = e >> 3, half = (e >> 2) & 1, q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-        float rowsum = 0.f;
-        for (int i = g; i < n_tiles; i += 2) {
-            const int b = g;
-            const uint32_t par = (i >> 1) & 1;
-            mbar_wait(&s_full[b], par);
-            tc_fence_after();
-            uint32_t v[32], lo[32];
-            tmem_ld32(lane_base + COL_S + b * BN + half * 32, v);
-            tc_fence_before();
-            mbar_arrive(&s_free[b]);                             // GEMM1 of tile i+2 may overwrite S now
-            const int64_t col = (int64_t)(t0 + i) * BN + half * 32;
-            if (col + 32 <= n_c) exp_chunk<false>(v, lo, offset, colscale, col, n_c, rowsum);
-            else exp_chunk<true>(v, lo, offset, colscale, col, n_c, rowsum);
-            mbar_wait(&e_free[b], par ^ 1);                      // GEMM2 of tile i-2 has consumed the previous E
-            tc_fence_after();
-            tmem_st32(lane_base + COL_EHI + b * BN + half * 32, v);
-            tmem_st32(lane_base + COL_ELO + b * BN + half * 32, lo);
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            mbar_arrive(&e_ready[b]);
-        }
-        // ---- combine the four sub-groups' row sums; group 0 reads O out of TMEM once per CTA ----
-        const int sub = g * 2 + half;
-        if (sub > 0) rowsum_x[(sub - 1) * 128 + row] = rowsum;
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        if (g == 0) {
-            mbar_wait(o_full, 0);
-            tc_fence_after();
-            const int64_t grow = (int64_t)row0 + row;
-            if (half < D / 32) {
-                if (n_tiles > 0) {
-                    uint32_t v[32], c[32];
-                    tmem_ld32(lane_base + COL_O + half * 32, v);
-                    tmem_ld32(lane_base + COL_OC + half * 32, c);
-                    if (grow < n_r) {
-                        float4 *dst = reinterpret_cast<float4 *>(o_part + ((size_t)sp * n_r + grow) * D + half * 32);
-#pragma unroll
-                        for (int k = 0; k < 8; ++k)
-                            dst[k] = make_float4(__uint_as_float(v[4 * k]) + __uint_as_float(c[4 * k]),
-                                                 __uint_as_float(v[4 * k + 1]) + __uint_as_float(c[4 * k + 1]),
-                                                 __uint_as_float(v[4 * k + 2]) + __uint_as_float(c[4 * k + 2]),
-                                                 __uint_as_float(v[4 * k + 3]) + __uint_as_float(c[4 * k + 3]));
-                    }
-                } else if (grow < n_r) {
-                    for (int k = 0; k < 32; ++k) o_part[((size_t)sp * n_r + grow) * D + half * 32 + k] = 0.f;
-                }
-            }
-            if (half == 0 && grow < n_r && rowsum_part != nullptr)
-                rowsum_part[(size_t)sp * n_r + grow] = rowsum + rowsum_x[row] + rowsum_x[128 + row] + rowsum_x[256 + row];
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemCols) : "memory");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    // ===================== consumers: rows [64 * (wg - 1), +64) of the R tile =====================
+    const int w = (threadIdx.x >> 5) & 3, g = lane >> 2, t = lane & 3;
+    const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;      // this warpgroup's 64 rows inside each R chunk
+    const uint32_t r_hi_a = smem_u32(r_hi) + a_off, r_lo_a = smem_u32(r_lo) + a_off;
+    float o[D / 2], oc[D / 2], sacc[32];
+    uint32_t ahi[32], alo[32];
+#pragma unroll
+    for (int k = 0; k < D / 2; ++k) o[k] = oc[k] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) {
+        sacc[k] = 0.f;
+        ahi[k] = alo[k] = 0u;
+    }
+    float rowsum[2] = {0.f, 0.f};
+    mbar_wait(r_full, 0);
+    for (int i = 0; i < n_tiles; ++i) {
+        const int s = i % ST;
+        mbar_wait(&full[s], (i / ST) & 1);
+        const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::C_BYTES;
+        const uint32_t t_hi_a = c_lo_a + K::C_BYTES, t_lo_a = t_hi_a + K::T_BYTES;
+        // ---- GEMM1: S = R C^T, three tf32 products, the small ones first ----
+        wg_fence();
+#pragma unroll
+        for (int part = 0; part < 3; ++part) {
+            const uint32_t ra = (part == 0) ? r_lo_a : r_hi_a;
+            const uint32_t cb = (part == 1) ? c_lo_a : c_hi_a;
+#pragma unroll
+            for (int kk = 0; kk < D / 8; ++kk) {
+                const uint32_t koff = (kk & 3) * 32;
+                wgmma_ss_n64(sacc, wg_desc(ra + (kk >> 2) * K::R_CHUNK + koff), wg_desc(cb + (kk >> 2) * K::C_CHUNK + koff),
+                             (part > 0 || kk > 0) ? 1u : 0u);
+            }
+        }
+        wg_commit();
+        wg_wait0();
+        reg_fence(sacc);
+        // ---- E = exp2(S - offset) * colscale, row sums, GEMM2's A fragment ----
+        const int64_t col0 = (int64_t)(t0 + i) * BN;
+        if (col0 + BN <= n_c) exp_tile<false>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
+        else exp_tile<true>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
+        // ---- GEMM2: O += E C (hi*hi into O, the two correction products into OC) ----
+        wg_fence();
+#pragma unroll
+        for (int part = 0; part < 3; ++part) {
+            const uint32_t *ea = (part == 0) ? alo : ahi;
+            const uint32_t tb = (part == 1) ? t_lo_a : t_hi_a;
+#pragma unroll
+            for (int kk = 0; kk < BN / 8; ++kk) {
+                const uint64_t bd = wg_desc(tb + (kk >> 2) * K::T_CHUNK + (kk & 3) * 32);
+                if (part == 2) wgmma_rs<D>(o, ea + 4 * kk, bd);
+                else wgmma_rs<D>(oc, ea + 4 * kk, bd);
+            }
+        }
+        wg_commit();
+        // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas; the other
+        // consumer warpgroup's MMAs fill the tensor pipe meanwhile
+        wg_wait0();
+        reg_fence(ahi);
+        reg_fence(alo);
+        reg_fence(o);
+        reg_fence(oc);
+        mbar_arrive(&empty[s]);                               // both copies of tile i are consumed
+    }
+
+    // ---- epilogue: o[4j + 2h + c] = O(row 16w + g + 8h, col 8j + 2t + c) ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
+        rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
+        const int64_t grow = (int64_t)row0 + (wg - 1) * 64 + 16 * w + g + 8 * h;
+        if (grow >= n_r) continue;
+        float *dst = o_part + ((size_t)sp * n_r + grow) * D;
+#pragma unroll
+        for (int j = 0; j < D / 8; ++j)
+            *reinterpret_cast<float2 *>(dst + 8 * j + 2 * t) =
+                make_float2(o[4 * j + 2 * h] + oc[4 * j + 2 * h], o[4 * j + 2 * h + 1] + oc[4 * j + 2 * h + 1]);
+        if (t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h];
     }
 }
 
@@ -475,9 +382,7 @@ int launch_tc(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_
     if ((rc = make_map(&mc_lo, C_lo, n_c, D, D, BN)) != SSL_OK) return rc;
     if ((rc = make_map(&mt_hi, CT_hi, D, n_c, ct_pitch, D)) != SSL_OK) return rc;
     if ((rc = make_map(&mt_lo, CT_lo, D, n_c, ct_pitch, D)) != SSL_OK) return rc;
-    constexpr int KCH = D / 32;
-    const size_t smem = 1024 + 2 * (size_t)KCH * BM * 128 + (size_t)ST1 * 2 * KCH * BN * 128 + (size_t)ST2 * 2 * (BN / 32) * D * 128 +
-                        32 * sizeof(uint64_t) + 16 + 3 * 128 * sizeof(float);
+    const size_t smem = Cfg<D>::SMEM;
     // cudaFuncSetAttribute is per DEVICE: remember which devices of this process are configured
     static bool configured[64] = {};
     int dev = 0;
@@ -507,6 +412,7 @@ extern "C" int ssl_softmax_gemm_tf32x3(const float *R_hi, const float *R_lo, int
                     reinterpret_cast<uintptr_t>(C_lo) | reinterpret_cast<uintptr_t>(CT_hi) | reinterpret_cast<uintptr_t>(CT_lo) |
                     reinterpret_cast<uintptr_t>(o_part)) & 15) == 0,
                   "ssl_softmax_gemm_tf32x3: operands must be 16-byte aligned");
+    SSL_CHECK_ARG((reinterpret_cast<uintptr_t>(colscale) & 7) == 0, "ssl_softmax_gemm_tf32x3: colscale must be 8-byte aligned");
     if (n_r == 0 || n_c == 0) return SSL_OK;
     cudaStream_t st = (cudaStream_t)stream;
     if (dim == 32) return launch_tc<32>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, st);

@@ -21,7 +21,7 @@
 // View-major variant (VM): with per-view inputs the grid's y dimension is the view and a thread
 // keeps one accumulator.  CTAs are scheduled x-fastest, so all rows of view 0 run before view 1:
 // the gathered working set is one view's rows (41 MB at the amazon shape) instead of the interleaved
-// [N, V, d] table (123 MB, which thrashed the 126 MB L2 at 57 % hits).
+// [N, V, d] table (123 MB, more than twice the 50 MB L2).
 #include <algorithm>
 #include <cmath>
 #include <string>
@@ -48,7 +48,7 @@ constexpr int kMinSeg = 128;       // rows up to this many entries are never spl
 constexpr int kThreads = 256;
 constexpr int kPartialStride = SSL_MAX_VIEWS * SSL_MAX_DIM;
 // ssl_set_option("prop_view_major", 1): one view per thread, grid.y = view -- DRAM traffic at 1.03x compulsory instead of 1.3x,
-// but 25-40 % slower on B200 (the kernel is issue / latency bound, not DRAM bound: profiles/r02_prop_variants.md).  Default off.
+// at the cost of less work per thread (the kernel is issue / latency bound, not DRAM bound).  Default off.
 bool g_view_major = false;
 
 struct PlanDev {

@@ -1,4 +1,4 @@
-"""Host-side orchestration of the sm_100a kernels: multi-view K-layer propagation (forward and
+"""Host-side orchestration of the sm_90a kernels: multi-view K-layer propagation (forward and
 the transposed backward), and the autograd plumbing that lets ``cal_loss`` read like the
 reference's while every gradient is accumulated in place by the kernels.
 
@@ -26,9 +26,10 @@ from ._lib import PropArgs, check, lib
 from .graph import GraphPlan
 
 LOG2E = 1.4426950408889634
-# InfoNCE contraction on tcgen05 (3xTF32, fp32-grade accuracy) when the dim allows; set to False to force the
-# FP32-FMA kernel (tests compare the two)
+# InfoNCE contraction on the wgmma tensor cores (3xTF32, fp32-grade accuracy) when the dim allows; set to False to force
+# the FP32-FMA kernel (tests compare the two)
 USE_TENSOR_CORES = True
+NUM_SM = 132          # H100 SXM; grids of the contraction are sized in resident-CTA slots (kNumSM in csrc/common.cuh)
 
 
 def _stream(t: torch.Tensor) -> int:
@@ -686,14 +687,14 @@ def bpr_loss_sum(users: Rows, items: Rows, ancs, poss, negs) -> torch.Tensor:
     return _BprFn.apply(users, items, ancs, poss, negs, *_tokens(users, items))
 
 
-def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * 148, prefer_few: bool = False) -> int:
+def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_few: bool = False) -> int:
     """Number of chunks the streamed operand is cut into: n_rtiles * n_split CTAs on ``slots`` resident-CTA slots (2 per SM for
-    the FFMA kernel at dim <= 64, 1 per SM for the tcgen05 kernel), every CTA keeping >= 4 tiles.
+    the FFMA kernel at dim <= 64, 1 per SM for the tensor-core kernel), every CTA keeping >= 4 tiles.
 
-    ``prefer_few`` (the tcgen05 kernel): minimise  waves(s) * (tiles_per_cta(s) + c)  with c = 5.5 tile-times of per-CTA overhead
-    (resident-tile load, TMEM allocation, pipeline fill, O read-out), fitted to a sweep on B200 at the bench shapes (tools/perf_tc.py
-    sweep, profiles/r02_ncu_kernels.md): forward role 32 row tiles x 1195 tiles -> 9 (0.314 ms; 5: 0.518, 14: 0.391); backward role
-    598 row tiles x 64 tiles -> 2 (0.357 ms; the pure wave-efficiency rule picked 4: 0.390).
+    ``prefer_few`` (the tensor-core kernel): minimise  waves(s) * (tiles_per_cta(s) + c)  with c = 5.5 tile-times of per-CTA
+    overhead (resident-tile load, pipeline fill, O write-out); fewer, longer CTAs than the pure wave-efficiency rule picks.
+    c was fitted to the contraction kernel this wgmma kernel replaced and has not been re-measured for it (a sweep:
+    tools/perf_tc.py sweep); the split only changes how the work is cut, never the result beyond summation order.
     Otherwise: the split with the best wave efficiency (FFMA kernel)."""
     max_split = max(1, min(n_ctiles // 4 if n_ctiles >= 4 else 1, 64))
     if prefer_few:
@@ -726,7 +727,7 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
         table = table.sub(lo, hi)
         n = table.n
         npad = max(64, ceil_to(n, 64))
-    use_tc = USE_TENSOR_CORES and d in (32, 64)     # tcgen05 3xTF32 contraction; other dims run the FFMA kernel
+    use_tc = USE_TENSOR_CORES and d in (32, 64)     # tensor-core 3xTF32 contraction; other dims run the FFMA kernel
     t_hat, rinv_t = torch.empty(npad, d, **f), torch.empty(max(n, 1), **f)
     if use_tc:
         a_t = t_t = None
@@ -735,7 +736,7 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
     else:
         t_t = torch.empty(npad // 64, d, 64, **f)
         a_hi = a_lo = t_hi = t_lo = a_thi = a_tlo = t_thi = t_tlo = None
-    n_split = choose_split((B + 127) // 128, npad // 64, slots=148 if use_tc else 296, prefer_few=use_tc)
+    n_split = choose_split((B + 127) // 128, npad // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
     rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
     rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
     off = LOG2E / tau
@@ -792,7 +793,7 @@ def _nce_bwd(saved, g):
         if gt is not None and n > 0:
             colscale = torch.zeros(ceil_to(B, 64), **f)   # padded tail is read (then masked) by the tile loads
             check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), scale, colscale.data_ptr(), s), 'ssl_nce_colscale')
-            n_split = choose_split((n + 127) // 128, ceil_to(B, 64) // 64, slots=148 if tc else 296, prefer_few=bool(tc))
+            n_split = choose_split((n + 127) // 128, ceil_to(B, 64) // 64, slots=NUM_SM if tc else 2 * NUM_SM, prefer_few=bool(tc))
             dt_part = torch.empty(n_split, n, d, **f)
             with _timed('nce_gemm_bwd', dict(B=B, n=n, dim=d, tc=bool(tc))):
                 if tc:
@@ -881,7 +882,7 @@ class _DenseLseFn(torch.autograd.Function):
         A = _raw_operand(a, LOG2E / temp, use_tc)
         T = _raw_operand(t, 1.0, use_tc)
         f = dict(device=a.device, dtype=torch.float32)
-        n_split = choose_split((B + 127) // 128, T[6] // 64, slots=148 if use_tc else 296, prefer_few=use_tc)
+        n_split = choose_split((B + 127) // 128, T[6] // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
         rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
         rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
         with torch.cuda.device(a.device):
@@ -904,7 +905,7 @@ class _DenseLseFn(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             f = dict(device=g.device, dtype=torch.float32)
             colscale = torch.zeros(A[6], **f)
-            n_split = choose_split((n + 127) // 128, A[6] // 64, slots=148 if use_tc else 296, prefer_few=use_tc)
+            n_split = choose_split((n + 127) // 128, A[6] // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
             dt_part = torch.empty(n_split, n, d, **f)
             with torch.cuda.device(g.device):
                 s = _stream(g)
@@ -982,7 +983,7 @@ def _uniform_fwd(x: Rows, ix):
     r, _, (r_hi, r_lo, _, _, _) = _unit_rows(x, ix, off, False, use_tc)
     c, rinv, (c_hi, c_lo, c_thi, c_tlo, c_t) = _unit_rows(x, ix, 1.0, True, use_tc)
     f = dict(device=dev, dtype=torch.float32)
-    n_split = choose_split((B + 127) // 128, Bp // 64, slots=148 if use_tc else 296, prefer_few=use_tc)
+    n_split = choose_split((B + 127) // 128, Bp // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
     rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
     pair_sum, w, total = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty((), **f)
     with torch.cuda.device(dev):

@@ -1,4 +1,4 @@
-"""HCCF -- drop-in for models/general_cf/hccf.py.  The GCN half of every layer is the sm_100a SpMM
+"""HCCF -- drop-in for models/general_cf/hccf.py.  The GCN half of every layer is the sm_90a SpMM
 with a fresh, rescaled in-kernel edge mask (hccf.py:33,47); the two contrastive terms per layer and
 side run through the fused InfoNCE kernels (loss_utils.py:42-51); the hyper-graph half
 (E W, H^T X, H . : skinny [N_side, d] x [d, hyper_num] products with dropout and LeakyReLU, hccf.py:43-49,100-108)

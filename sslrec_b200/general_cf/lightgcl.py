@@ -2,10 +2,10 @@
 
 The reference keeps a U x I matrix R / sqrt(rowD colD) and propagates users and items with two scatter
 ``_spmm`` calls per layer (lightgcl.py:59-66,75-76).  Stacked as the symmetric bipartite matrix that pair
-is one launch of the sm_100a SpMM, [Z_u; Z_i] = A [E_u; E_i], with the dropout of the stored values
+is one launch of the sm_90a SpMM, [Z_u; Z_i] = A [E_u; E_i], with the dropout of the stored values
 (``_sparse_dropout``, :68-72) evaluated in-kernel per layer and direction.  The low-rank branch
 (U S)(V^T E), (V S)(U^T E) (:79-83) is two skinny library GEMMs per side; the contrastive term's
-log sum_j exp(G[b] . E_j / temp) over ALL users / items (:112-113) runs on the tcgen05 contraction without the
+log sum_j exp(G[b] . E_j / temp) over ALL users / items (:112-113) runs on the tensor-core contraction without the
 [B, N] logits (engine.dense_logsumexp_mean).  Layers are tied together by torch autograd, as in HCCF."""
 from __future__ import annotations
 

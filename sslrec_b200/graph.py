@@ -1,6 +1,6 @@
 """Adjacency plan: the reference's ``data_handler.torch_adj`` (an uncoalesced, column-sorted COO
 fp32 tensor, data_utils/data_handler_general_cf.py:53-73) converted ONCE to the int32 CSR the
-sm_100a propagation kernel walks.  The structure and the values are symmetric (D^-1/2 A D^-1/2
+sm_90a propagation kernel walks.  The structure and the values are symmetric (D^-1/2 A D^-1/2
 of an undirected bipartite graph), so the same CSR serves the forward SpMM and the transposed
 SpMM of the backward pass; only an *injected* edge mask needs the reverse-entry permutation.
 """

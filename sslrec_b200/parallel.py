@@ -111,9 +111,8 @@ class RowShard:
             raise ValueError("transport must be 'symm' (fused NVLink stores) or 'nccl' (all_gather after the launch)")
         self.transport = transport
         # symm transport, optional: store finished rows ONCE, to the NVSwitch multicast address of the table (the switch
-        # replicates; the sender's egress drops by world - 1) instead of once per peer.  Measured on 8 x B200 at BASELINE
-        # config 4 (profiles/r02_multi_gpu.md): no faster (57.9 vs 57.7 ms of SpMM per step) -- the exchange is bound by what every
-        # GPU RECEIVES (5.4 GB per layer), not by what it sends -- so the plain peer stores stay the default.
+        # replicates; the sender's egress drops by world - 1) instead of once per peer.  The exchange is bound by what every GPU
+        # RECEIVES, not by what it sends, so the plain peer stores stay the default.
         # multicast=True or SSLREC_B200_MULTICAST=1 selects it.
         import os
         env = os.environ.get('SSLREC_B200_MULTICAST')

@@ -11,8 +11,8 @@ SHAPES = {
     'gowalla': (25557, 19747, 294983),
     'yelp': (42712, 26822, 182357),
     'amazon': (76469, 83761, 966680),
-    'synthetic-xl': (10_000_000, 2_000_000, 300_000_000),
-    'synthetic-xl-8th': (1_250_000, 250_000, 37_500_000),      # one GPU's eighth of config 4 (same degree statistics)
+    'synthetic-xl': (5_000_000, 1_000_000, 150_000_000),       # config 4: the whole graph trains on one 80 GB GPU
+    'synthetic-xl-8th': (625_000, 125_000, 18_750_000),      # one GPU's eighth of config 4 (same degree statistics)
 }
 # item-popularity exponent: 0.5 reproduces the bundled datasets' head (max item degree ~1e3 at
 # amazon's size; the real matrices have 841 / 309 / 1018); 1.0 is BASELINE.json config 4's generator
@@ -72,7 +72,7 @@ def bipartite_graph(n_user: int, n_item: int, n_edge: int, seed: int = 2023, zip
 
 # --------------------------------------------------------------------------------------------------
 # The same family of graphs generated ON THE DEVICE (torch CUDA ops), for BASELINE.json config 4
-# (10 M x 2 M nodes, 300 M edges): the numpy path above needs minutes and tens of GB of host memory
+# (5 M x 1 M nodes, 150 M edges): the numpy path above needs minutes and tens of GB of host memory
 # at that size, the device path a few seconds.  Same distributions (lognormal user degrees, Zipf item
 # popularity over a random permutation, duplicates removed, exactly n_edge pairs), torch's Philox
 # generator with a fixed seed -- NOT bit-identical to the numpy generator.

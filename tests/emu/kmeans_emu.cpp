@@ -1,4 +1,4 @@
-// Host execution of sslrec_b200/csrc/kmeans_assign.cuh (the SAME source the library compiles for sm_100a): the R = 4 instantiation
+// Host execution of sslrec_b200/csrc/kmeans_assign.cuh (the SAME source the library compiles for sm_90a): the R = 4 instantiation
 // against the R = 1 one (bit for bit: assignments, per-CTA partial sums and counts, change counter) and against a plain restatement
 // of one Lloyd assignment pass (aug_utils.py:150-155).  usage: kmeans_emu n dim K n_cta W seed
 #include <stdio.h>

@@ -1,4 +1,4 @@
-// Host execution of sslrec_b200/csrc/predict_tile.cuh (the SAME source the library compiles for sm_100a) against a float64
+// Host execution of sslrec_b200/csrc/predict_tile.cuh (the SAME source the library compiles for sm_90a) against a float64
 // restatement of base_model.py:35-36 + lightgcn.py:64.  usage: predict_emu n_b n_item dim u_stride i_stride mode seed
 //   mode 0: no mask, 1: dense int64 mask, 2: training CSR
 #include <stdio.h>

@@ -59,7 +59,7 @@ def make_scratch_tree():
     return d
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REFDIR, 'models')), reason='oracle/_ref not vendored (python oracle/vendor_ref.py in the build container)')
+@pytest.mark.skipif(not os.path.isdir(os.path.join(REFDIR, 'models')), reason='oracle/_ref not vendored (python oracle/vendor_ref.py)')
 def test_scratch_tree_overlays_only_the_shims():
     d = make_scratch_tree()
     gc = os.path.join(d, 'models', 'general_cf')

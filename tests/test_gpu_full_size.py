@@ -256,8 +256,8 @@ def test_hccf_amazon_shape_h128_matches_oracle():
 
 
 def test_lightgcn_config4_slice_d128_matches_oracle():
-    """The d = 128 path of BASELINE config 4 on a 1/16 slice of its graph family (625 k x 125 k nodes, 18.75 M edges: the
-    384 MB table is 3x the L2): propagation + BPR + reg forward and backward against the oracle."""
+    """The d = 128 path of BASELINE config 4 on a 1/8 slice of its graph family (625 k x 125 k nodes, 18.75 M edges: the
+    384 MB table is 8x the 50 MB L2): propagation + BPR + reg forward and backward against the oracle."""
     import synth_graphs as S
     U, I, E = 625_000, 125_000, 18_750_000
     keys = S.bipartite_keys_device(U, I, E, 2023, 1.0, 'cuda')

@@ -145,7 +145,7 @@ def test_node_drop_forward_backward():
 @pytest.mark.parametrize('use_tc', [True, False])
 @pytest.mark.parametrize('dim,B,n', [(64, 4096, 9000), (32, 100, 777), (128, 300, 2000), (48, 257, 1000), (64, 64, 50), (64, 130, 64 * 9 + 1)])
 def test_infonce_term_forward_backward(dim, B, n, use_tc, monkeypatch):
-    """use_tc: the tcgen05 3xTF32 contraction (dims 32 / 64) vs the FP32-FMA kernel -- same tolerances."""
+    """use_tc: the tensor-core 3xTF32 contraction (dims 32 / 64) vs the FP32-FMA kernel -- same tolerances."""
     from sslrec_b200 import engine
     from sslrec_b200 import loss_utils as LU
     monkeypatch.setattr(engine, 'USE_TENSOR_CORES', use_tc)
@@ -161,9 +161,8 @@ def test_infonce_term_forward_backward(dim, B, n, use_tc, monkeypatch):
     ref = O.infonce_loss_sum(*ref_in, tau)
     ref.backward()
     assert abs(loss.item() - ref.item()) <= 2e-6 * abs(ref.item())
-    # absolute term relative to the largest gradient entry: 2e-6 for the FP32-FMA kernel; 1e-5 for the tcgen05
-    # 3xTF32 kernel, whose tensor-core accumulators round toward zero over up to ~10^3 accumulations per output
-    # (measured 0.5-2.5e-6 of the largest entry, tools/debug_tc.py)
+    # absolute term relative to the largest gradient entry: 2e-6 for the FP32-FMA kernel; 1e-5 for the tensor-core
+    # 3xTF32 kernel, whose tensor-core accumulators do not round to nearest over up to ~10^3 accumulations per output
     rel_atol = 1e-5 if (use_tc and dim in (32, 64)) else 2e-6
     for a, b, name in zip(ins, ref_in, ('e1', 'e2', 'table')):
         H.close(a.grad, b.grad, 2e-4, rel_atol * b.grad.abs().max().item(), 'grad ' + name)
@@ -465,7 +464,7 @@ def test_kmeans_matches_oracle_and_is_deterministic(n, dim, K):
 @pytest.mark.parametrize('dim,B', [(64, 4096), (32, 100), (128, 300), (48, 257), (64, 2)])
 def test_alignment_uniformity_forward_backward(dim, B, use_tc, monkeypatch):
     """DirectAU's losses (loss_utils.py:75-86) with the reference's dense signatures against the float64 oracle;
-    the uniformity pair sum runs on the InfoNCE contraction (tcgen05 3xTF32 at dims 32 / 64, FP32 FMA otherwise)."""
+    the uniformity pair sum runs on the InfoNCE contraction (tensor-core 3xTF32 at dims 32 / 64, FP32 FMA otherwise)."""
     from sslrec_b200 import engine
     from sslrec_b200 import loss_utils as LU
     monkeypatch.setattr(engine, 'USE_TENSOR_CORES', use_tc)

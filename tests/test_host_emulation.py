@@ -1,5 +1,5 @@
 """Kernel sources executed ON THE HOST.  The tiled score kernel (sslrec_b200/csrc/predict_tile.cuh): the same source the library compiles for
-sm_100a, run thread by thread (tests/emu/cuda_emu.h: one pthread per CUDA thread, __syncthreads = barrier) under
+sm_90a, run thread by thread (tests/emu/cuda_emu.h: one pthread per CUDA thread, __syncthreads = barrier) under
 AddressSanitizer, against a float64 restatement of lightgcn.py:64 + base_model.py:35-36 and bit for bit against the sequential
 fp32 FMA chain the kernel documents.  Every global / shared-memory index the kernel forms is checked at ragged sizes (tiles cut
 by n_b and n_item, inner dimensions that are not a multiple of the staging depth, strided tables, repeated users), for the

@@ -1,7 +1,7 @@
 // Roofline denominators of the SpMM gather: random row gathers (256 B and 512 B rows, as prop_kernel issues them:
 // one float4 per lane, 8 rows in flight per group) from tables that fit the L2 (16 .. 96 MB) and that do not
 // (384 MB .. 6 GB).  Prints one JSON object per (row bytes, table size): GB/s of gathered bytes.
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/gather_bench tools/gather_bench.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/gather_bench tools/gather_bench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -45,7 +45,7 @@ void run(size_t table_mb, int64_t n_gather) {
     for (int64_t i = 0; i < n_gather; ++i) { s ^= s << 13; s ^= s >> 7; s ^= s << 17; h[i] = (int32_t)(s % n_rows); }
     CK(cudaMemcpy(idx, h, n_gather * 4, cudaMemcpyHostToDevice)); free(h);
     cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    const int grid = 148 * 4 * 8;
+    const int grid = 132 * 4 * 8;
     for (int i = 0; i < 3; ++i) gather_kernel<G><<<grid, 256>>>(table, idx, n_gather, sink);
     CK(cudaDeviceSynchronize());
     float best = 1e30f, tot = 0.f;

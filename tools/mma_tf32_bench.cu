@@ -37,22 +37,22 @@ __global__ void ffma_loop(float *out, int iters) {
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 int main() {
-    float *out; cudaMalloc(&out, 148 * 8 * 256 * 4);
+    float *out; cudaMalloc(&out, 132 * 8 * 256 * 4);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int threads : {128, 256, 512}) for (int bps : {1, 2, 4}) {
         int iters = 20000; float ms;
-        mma_loop<<<148 * bps, threads>>>(out, 100); cudaDeviceSynchronize();
-        cudaEventRecord(e0); mma_loop<<<148 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
+        mma_loop<<<132 * bps, threads>>>(out, 100); cudaDeviceSynchronize();
+        cudaEventRecord(e0); mma_loop<<<132 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
-        double fl = 148.0 * bps * (threads / 32) * (double)iters * 8 * 2.0 * 16 * 8 * 8;
+        double fl = 132.0 * bps * (threads / 32) * (double)iters * 8 * 2.0 * 16 * 8 * 8;
         printf("mma.sync tf32 m16n8k8 : %3d thr x %d blk/SM: %.1f TFLOP/s\n", threads, bps, fl / ms / 1e9);
-        cudaEventRecord(e0); mma_bf16_loop<<<148 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
+        cudaEventRecord(e0); mma_bf16_loop<<<132 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
-        fl = 148.0 * bps * (threads / 32) * (double)iters * 8 * 2.0 * 16 * 8 * 16;
+        fl = 132.0 * bps * (threads / 32) * (double)iters * 8 * 2.0 * 16 * 8 * 16;
         printf("mma.sync bf16 m16n8k16: %3d thr x %d blk/SM: %.1f TFLOP/s\n", threads, bps, fl / ms / 1e9);
-        cudaEventRecord(e0); ffma_loop<<<148 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
+        cudaEventRecord(e0); ffma_loop<<<132 * bps, threads>>>(out, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
         cudaEventElapsedTime(&ms, e0, e1);
-        fl = 148.0 * bps * threads * (double)iters * 32 * 2.0;
+        fl = 132.0 * bps * threads * (double)iters * 32 * 2.0;
         printf("ffma                  : %3d thr x %d blk/SM: %.1f TFLOP/s\n", threads, bps, fl / ms / 1e9);
     }
     printf("cuda error: %s\n", cudaGetErrorString(cudaGetLastError()));

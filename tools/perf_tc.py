@@ -3,6 +3,7 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from sslrec_b200._lib import lib, check
+from sslrec_b200 import engine as E
 from sslrec_b200.engine import choose_split
 f = dict(device='cuda', dtype=torch.float32)
 def prep(x, n, d, alpha):
@@ -14,7 +15,7 @@ def prep(x, n, d, alpha):
 def run(nr, nc, d, tc, reps=10, split=None):
     g = torch.Generator().manual_seed(0)
     R = prep(torch.randn(nr, d, generator=g).cuda(), nr, d, 7.2); C = prep(torch.randn(nc, d, generator=g).cuda(), nc, d, 1.0)
-    ns = split or choose_split((nr + 127) // 128, C[6] // 64, slots=148 if tc else 296, prefer_few=tc)
+    ns = split or choose_split((nr + 127) // 128, C[6] // 64, slots=E.NUM_SM if tc else 2 * E.NUM_SM, prefer_few=tc)
     rs, o = torch.zeros(ns, nr, **f), torch.zeros(ns, nr, d, **f)
     s = torch.cuda.current_stream().cuda_stream
     def call():

@@ -44,7 +44,7 @@ def main():
     shapes['bwd last layer (reduce over views; interleaved only)'] = (plain, e_)
     # the HBM-bound regime: one GPU's eighth of BASELINE config 4 (1.5 M nodes, 75 M entries, d = 128, one view)
     if '--xl' in sys.argv or '--xlfull' in sys.argv:
-        sc = 8 if '--xlfull' in sys.argv else 1            # --xlfull: the whole BASELINE config 4 (12 M nodes, 600 M entries, 6.1 GB table)
+        sc = 8 if '--xlfull' in sys.argv else 1            # --xlfull: the whole BASELINE config 4 (6 M nodes, 300 M entries, 3.1 GB table)
         nu_x, ni_x = 1_250_000 * sc, 250_000 * sc
         keys = S.bipartite_keys_device(nu_x, ni_x, 37_500_000 * sc, 2023, 1.0, 'cuda')
         rp, ci, va = S.normalized_csr_device(keys, nu_x, ni_x)

@@ -1,4 +1,4 @@
-"""HBM-bound measurement of the propagation kernel: a graph whose table is far larger than the 126 MB L2
+"""HBM-bound measurement of the propagation kernel: a graph whose table is far larger than the 50 MB L2
 (BASELINE.json config 4's per-GPU regime), forward layer launches timed with CUDA events on the launching stream.
 Usage (GPU box): python tools/spmm_roofline.py [n_nodes] [avg_degree] [dim] [views]"""
 import json, os, sys, time
