@@ -206,7 +206,8 @@ SSL_API int ssl_bpr_bwd(const float *users, int64_t u_stride, const float *items
  *   rinv [n] (the 1/norm used, needed by the backward), and optionally the tf32 split
  *   out_hi = tf32(out), out_lo = out - out_hi, row-major [n, dim] each, plus their transposes
  *   out_thi / out_tlo [dim, t_pitch] (t_pitch >= ceil64(n), multiple of 4) that
- *   ssl_softmax_gemm_tf32x3 reads through TMA.
+ *   ssl_softmax_gemm_tf32x3 reads through TMA, with the columns of every aligned group of 8 stored
+ *   in the order 0 2 4 6 1 3 5 7 (row 8j + 2t + c at column 8j + t + 4c) and rows n .. ceil64(n) zero.
  * ssl_softmax_gemm    for every row r of R [n_r, dim] over the rows c of C (row-major C
  *   [n_c, dim] and its K-major tile copy C_t):   e = exp2(R_r . C_c - offset) * colscale[c]
  *   rowsum_part[s, r] = sum_c e   (optional)     o_part[s, r, :] = sum_c e * C_c
@@ -223,7 +224,8 @@ SSL_API int ssl_softmax_gemm(const float *R, int64_t n_r, const float *C, const 
                      void *stream);
 /* The same contraction on the Hopper tensor cores (wgmma) with 3xTF32 error compensation (fp32-grade
  * accuracy): operands are the hi / lo splits written by ssl_rows_normalize, row-major [n, dim],
- * and for the streamed operand also the transposed splits CT_hi / CT_lo [dim, ct_pitch];
+ * and for the streamed operand also the transposed splits CT_hi / CT_lo [dim, ct_pitch] in
+ * ssl_rows_normalize's column order (ct_pitch >= ceil8(n_c), columns n_c .. ceil8(n_c) zero);
  * dim must be 32 or 64.  colscale, when given, must be readable up to ceil64(n_c) floats (the
  * padded tail is loaded with the tile and masked).  Outputs and semantics are those of
  * ssl_softmax_gemm. */

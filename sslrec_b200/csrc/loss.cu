@@ -127,13 +127,16 @@ __global__ void __launch_bounds__(256) rows_normalize_kernel(const float *__rest
             dst[i] = tile[c * pitch + k];
         }
     }
-    if (out_thi != nullptr) {       // transposed tf32 split: [dim, t_pitch], 64 consecutive columns per block
+    if (out_thi != nullptr) {       // transposed tf32 split: [dim, t_pitch], 64 columns per block
+        // within every group of 8 columns, row 8j + 2t + c goes to column 8j + t + 4c: the order in which the tensor-core
+        // contraction holds E in its accumulator fragment, so that fragment feeds the second GEMM's A operand unpermuted
         for (int i = threadIdx.x; i < dim * 64; i += 256) {
             const int k = i >> 6, c = i & 63;
+            const int q = (c & ~7) | ((c & 7) >> 1) | ((c & 1) << 2);
             float hi, lo;
             ssl::tf32_split(tile[c * pitch + k], hi, lo);
-            out_thi[(size_t)k * t_pitch + row0 + c] = hi;
-            out_tlo[(size_t)k * t_pitch + row0 + c] = lo;
+            out_thi[(size_t)k * t_pitch + row0 + q] = hi;
+            out_tlo[(size_t)k * t_pitch + row0 + q] = lo;
         }
     }
 }

@@ -10,18 +10,24 @@
 // dropped lo*lo products and the rounding of the lo parts are O(2^-22) relative and unbiased -- the fp32
 // rounding level of the FFMA kernel.
 //
-// Structure (one CTA per SM, 384 threads = 3 warpgroups, all synchronisation by mbarriers):
+// Structure (persistent: min(units, #SMs) CTAs of 384 threads = 3 warpgroups; a unit is one 128-row R tile against
+// one of the n_split chunks of C, and CTA b runs units b, b + gridDim.x, ... in that static order):
 //   warpgroup 0, one thread : TMA producer.  2-D tensor maps (SWIZZLE_128B, 32-float boxes) over the row-major
-//                     hi / lo operand arrays: the resident 128-row R tile once, then per 64-row C tile one ring
-//                     stage holding the row-major C tile (GEMM1's B operand) and the tile of the TRANSPOSED copy
-//                     [d, n] (GEMM2's B operand).  wgmma reads tf32 operands from shared memory K-major only,
-//                     which is why both copies are streamed.
-//   warpgroups 1, 2 : consumers, 64 rows of the R tile each, over all C tiles of the CTA:
-//                     GEMM1 (m64 n64 k8, both operands in shared memory) -> S in registers;  E = exp2(S - offset)
-//                     with the row sums in registers;  the accumulator fragment of S is permuted by warp shuffles
-//                     into the A-operand fragment of GEMM2 and split into tf32 hi / lo there;  GEMM2 (m64 nD k8,
-//                     A = E from registers, B = C^T tile) accumulates O.  The two warpgroups interleave their exp
-//                     phases with each other's MMAs.
+//                     hi / lo C arrays: per 64-row C tile one ring stage holding the row-major C tile (GEMM1's B
+//                     operand) and the tile of the TRANSPOSED copy [d, n] (GEMM2's B operand).  wgmma reads tf32
+//                     operands from shared memory K-major only, which is why both copies are streamed.  The ring
+//                     runs on across units, so the next unit's first tiles load under the current unit's last ones.
+//   warpgroups 1, 2 : consumers, 64 rows of the unit's R tile each.  At the start of a unit each thread loads its
+//                     R_hi / R_lo rows from global memory straight into the tf32 A fragment, so shared memory holds
+//                     only the C ring.  Per C tile: GEMM1 (m64 n64 k8, A = R from registers) -> S in registers;
+//                     E = exp2(S - offset) with the row sums in registers, split into tf32 hi / lo in place: the
+//                     accumulator fragment of S serves as GEMM2's A fragment as it is, because the transposed copy
+//                     holds its columns in the matching order (see exp_tile);
+//                     GEMM2 (m64 nD k8, A = E from registers, B = C^T tile) accumulates O, written out per unit.
+//                     Two named barriers hand the MMA issue back and forth (ping-pong), so one warpgroup's exp
+//                     phase runs under the other's MMAs.
+//   Units write disjoint o_part / rowsum_part slices and the order of every sum is fixed, so the output does not
+//   depend on the grid size or on timing.
 //   The two correction products of GEMM2 go to their own accumulator: the tensor core does not round its fp32
 //   accumulations to nearest, so the long hi*hi sum must not also carry them.
 #include <cuda.h>
@@ -37,11 +43,11 @@ constexpr int kNumThreads = 384;       // warpgroup 0: TMA producer; warpgroups 
 template <int D> struct Cfg {
     static constexpr int KCH = D / 32;                  // 128-byte K chunks per operand row (GEMM1: K = d)
     static constexpr int JCH = BN / 32;                 // 128-byte K chunks of the transposed tile (GEMM2: K = 64 rows)
-    static constexpr uint32_t R_CHUNK = BM * 128, C_CHUNK = BN * 128, T_CHUNK = D * 128;
-    static constexpr uint32_t R_BYTES = KCH * R_CHUNK, C_BYTES = KCH * C_CHUNK, T_BYTES = JCH * T_CHUNK;   // one precision part
+    static constexpr uint32_t C_CHUNK = BN * 128, T_CHUNK = D * 128;
+    static constexpr uint32_t C_BYTES = KCH * C_CHUNK, T_BYTES = JCH * T_CHUNK;   // one precision part
     static constexpr uint32_t STAGE_BYTES = 2 * C_BYTES + 2 * T_BYTES;
-    static constexpr int ST = (D == 32) ? 4 : 2;        // ring stages: 64 KB R + 2 x 64 KB at d = 64, 32 KB R + 4 x 32 KB at d = 32
-    static constexpr size_t SMEM = 1024 + 2 * (size_t)R_BYTES + (size_t)ST * STAGE_BYTES + (2 * ST + 1) * sizeof(uint64_t);
+    static constexpr int ST = (D == 32) ? 6 : 3;        // ring stages: 3 x 64 KB at d = 64, 6 x 32 KB at d = 32
+    static constexpr size_t SMEM = 1024 + (size_t)ST * STAGE_BYTES + 2 * ST * sizeof(uint64_t);
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -85,6 +91,9 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t addr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// named barriers over the two consumer warpgroups (256 threads); id 0 is __syncthreads'
+__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
 // keeps registers an asynchronous wgmma reads or writes live (and in place) up to this point
 template <int N>
 __device__ __forceinline__ void reg_fence(float (&r)[N]) {
@@ -97,21 +106,21 @@ __device__ __forceinline__ void reg_fence(uint32_t (&r)[N]) {
     for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
-// d[64 x 64] (+)= A[smem] * B[smem]^T
-__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+// d[64 x 64] (+)= A[registers, one k8 block] * B[smem]^T
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t *a, uint64_t b, uint32_t acc) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %34, 0;\n"
+        "setp.ne.b32 p, %37, 0;\n"
         "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-        "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n"
+        "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n"
         "}\n"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
           "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
           "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
           "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(a), "l"(b), "r"(acc));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }
 // d[64 x 64] += A[registers, one k8 block] * B[smem]^T
 __device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t *a, uint64_t b) {
@@ -141,14 +150,13 @@ __device__ __forceinline__ void wgmma_rs(float (&d)[D / 2], const uint32_t *a, u
 }
 
 // One 64-column tile of S (accumulator fragment: s[4j + 2h + c] = S(row g + 8h, col 8j + 2t + c), g = lane / 4,
-// t = lane % 4) -> E, the two row sums, and E as GEMM2's A fragment in tf32 hi / lo: a[4j + h] = E(g + 8h, 8j + t),
-// a[4j + 2 + h] = E(g + 8h, 8j + t + 4).  The column permutation is a shuffle among the four lanes of a row group.
+// t = lane % 4) -> E, the two row sums, and E as GEMM2's A fragment in tf32 hi / lo: a[4j + 2c + h] = E(g + 8h, 8j + 2t + c).
+// The A fragment's k index 8j + t + 4c thus stands for column 8j + 2t + c; ssl_rows_normalize writes the transposed copy
+// (GEMM2's B operand) in that column order, so no lane exchange is needed.
 template <bool CHECK>
 __device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[32], uint32_t (&alo)[32], float offset,
                                          const float *__restrict__ cs_ptr, int64_t col0, int64_t n_c, float (&rowsum)[2]) {
-    const int lane = threadIdx.x & 31, t = lane & 3;
-    const int src1 = (lane & ~3) | (t >> 1), src2 = src1 + 2;
-    const bool odd = (t & 1) != 0;
+    const int t = threadIdx.x & 3;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int64_t col = col0 + 8 * j + 2 * t;
@@ -171,13 +179,11 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[3
                 e1 = (col + 1 < n_c) ? e1 : 0.f;
             }
             rowsum[h] += e0 + e1;
-            const float v0 = __shfl_sync(0xffffffffu, e0, src1), v1 = __shfl_sync(0xffffffffu, e1, src1);
-            const float w0 = __shfl_sync(0xffffffffu, e0, src2), w1 = __shfl_sync(0xffffffffu, e1, src2);
             float hi, lo;
-            ssl::tf32_split(odd ? v1 : v0, hi, lo);
+            ssl::tf32_split(e0, hi, lo);
             ahi[4 * j + h] = __float_as_uint(hi);
             alo[4 * j + h] = __float_as_uint(lo);
-            ssl::tf32_split(odd ? w1 : w0, hi, lo);
+            ssl::tf32_split(e1, hi, lo);
             ahi[4 * j + 2 + h] = __float_as_uint(hi);
             alo[4 * j + 2 + h] = __float_as_uint(lo);
         }
@@ -186,7 +192,7 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[3
 
 template <int D>
 __global__ void __launch_bounds__(kNumThreads, 1)
-softmax_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_r_hi, const __grid_constant__ CUtensorMap map_r_lo,
+softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__ R_lo,
                        const __grid_constant__ CUtensorMap map_c_hi, const __grid_constant__ CUtensorMap map_c_lo,
                        const __grid_constant__ CUtensorMap map_ct_hi, const __grid_constant__ CUtensorMap map_ct_lo,
                        int64_t n_r, int64_t n_c, const float *__restrict__ colscale, float offset, int n_split,
@@ -194,22 +200,15 @@ softmax_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_r_hi, const __gri
     using K = Cfg<D>;
     constexpr int ST = K::ST, KCH = K::KCH, JCH = K::JCH;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *r_hi = smem, *r_lo = smem + K::R_BYTES;
-    uint8_t *ring = smem + 2 * K::R_BYTES;               // stage s: C hi, C lo (row-major tile), C^T hi, C^T lo
-    uint64_t *full = reinterpret_cast<uint64_t *>(ring + ST * K::STAGE_BYTES);
-    uint64_t *empty = full + ST, *r_full = empty + ST;
+    uint8_t *ring = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t *full = reinterpret_cast<uint64_t *>(ring + ST * K::STAGE_BYTES);   // stage s: C hi, C lo (row-major tile), C^T hi, C^T lo
+    uint64_t *empty = full + ST;
 
     const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-    const int rt = blockIdx.x / n_split, sp = blockIdx.x % n_split;
     const int64_t n_ct = (n_c + BN - 1) / BN;
-    const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
-    const int n_tiles = t1 - t0;
-    const int row0 = rt * BM;
+    const int n_units = (int)((n_r + BM - 1) / BM) * n_split;     // unit u: R tile u / n_split, C chunk u % n_split
 
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_r_hi));
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_r_lo));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_hi));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_lo));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ct_hi));
@@ -218,118 +217,143 @@ softmax_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_r_hi, const __gri
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 256);
         }
-        mbar_init(r_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
     if (wg == 0) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
         if (threadIdx.x == 0) {
-            // ===================== TMA producer: R tile once, then per C tile its row-major and transposed copies =====================
-            mbar_expect_tx(r_full, 2 * K::R_BYTES);
-            for (int c = 0; c < KCH; ++c) {
-                tma_load_2d(r_hi + c * K::R_CHUNK, &map_r_hi, c * 32, row0, r_full);
-                tma_load_2d(r_lo + c * K::R_CHUNK, &map_r_lo, c * 32, row0, r_full);
-            }
-            for (int i = 0; i < n_tiles; ++i) {
-                const int s = i % ST;
-                mbar_wait(&empty[s], ((i / ST) & 1) ^ 1);
-                uint8_t *c_hi = ring + s * K::STAGE_BYTES, *c_lo = c_hi + K::C_BYTES;
-                uint8_t *ct_hi = c_lo + K::C_BYTES, *ct_lo = ct_hi + K::T_BYTES;
-                mbar_expect_tx(&full[s], K::STAGE_BYTES);
-                for (int c = 0; c < KCH; ++c) {
-                    tma_load_2d(c_hi + c * K::C_CHUNK, &map_c_hi, c * 32, (t0 + i) * BN, &full[s]);
-                    tma_load_2d(c_lo + c * K::C_CHUNK, &map_c_lo, c * 32, (t0 + i) * BN, &full[s]);
-                }
-                for (int c = 0; c < JCH; ++c) {
-                    tma_load_2d(ct_hi + c * K::T_CHUNK, &map_ct_hi, (t0 + i) * BN + c * 32, 0, &full[s]);
-                    tma_load_2d(ct_lo + c * K::T_CHUNK, &map_ct_lo, (t0 + i) * BN + c * 32, 0, &full[s]);
+            // ===================== TMA producer: per C tile of every unit its row-major and transposed copies =====================
+            // the ring runs on across units, so the next unit's first tiles load under the current unit's last ones
+            int it = 0;
+            for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+                const int sp = u % n_split;
+                const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
+                for (int tile = t0; tile < t1; ++tile, ++it) {
+                    const int s = it % ST;
+                    mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
+                    uint8_t *c_hi = ring + s * K::STAGE_BYTES, *c_lo = c_hi + K::C_BYTES;
+                    uint8_t *ct_hi = c_lo + K::C_BYTES, *ct_lo = ct_hi + K::T_BYTES;
+                    mbar_expect_tx(&full[s], K::STAGE_BYTES);
+                    for (int c = 0; c < KCH; ++c) {
+                        tma_load_2d(c_hi + c * K::C_CHUNK, &map_c_hi, c * 32, tile * BN, &full[s]);
+                        tma_load_2d(c_lo + c * K::C_CHUNK, &map_c_lo, c * 32, tile * BN, &full[s]);
+                    }
+                    for (int c = 0; c < JCH; ++c) {
+                        tma_load_2d(ct_hi + c * K::T_CHUNK, &map_ct_hi, tile * BN + c * 32, 0, &full[s]);
+                        tma_load_2d(ct_lo + c * K::T_CHUNK, &map_ct_lo, tile * BN + c * 32, 0, &full[s]);
+                    }
                 }
             }
         }
         return;
     }
 
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
-    // ===================== consumers: rows [64 * (wg - 1), +64) of the R tile =====================
-    const int w = (threadIdx.x >> 5) & 3, g = lane >> 2, t = lane & 3;
-    const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;      // this warpgroup's 64 rows inside each R chunk
-    const uint32_t r_hi_a = smem_u32(r_hi) + a_off, r_lo_a = smem_u32(r_lo) + a_off;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;\n" ::: "memory");
+    // ===================== consumers: rows [64 * cw, +64) of each unit's R tile =====================
+    const int cw = wg - 1, w = (threadIdx.x >> 5) & 3, g = lane >> 2, t = lane & 3;
+    // ping-pong: named barrier 1 + cw is this warpgroup's turn to issue MMAs.  Each warpgroup issues a GEMM, passes the turn
+    // and only then waits for it, so one warpgroup's exp phase runs under the other's MMAs.  Consumer 0 goes first.
+    const int bar_mine = 1 + cw, bar_other = 2 - cw;
+    if (cw == 1) named_arrive(1);
     float o[D / 2], oc[D / 2], sacc[32];
-    uint32_t ahi[32], alo[32];
-#pragma unroll
-    for (int k = 0; k < D / 2; ++k) o[k] = oc[k] = 0.f;
+    uint32_t rhi[D / 2], rlo[D / 2], ahi[32], alo[32];
 #pragma unroll
     for (int k = 0; k < 32; ++k) {
         sacc[k] = 0.f;
         ahi[k] = alo[k] = 0u;
     }
-    float rowsum[2] = {0.f, 0.f};
-    mbar_wait(r_full, 0);
-    for (int i = 0; i < n_tiles; ++i) {
-        const int s = i % ST;
-        mbar_wait(&full[s], (i / ST) & 1);
-        const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::C_BYTES;
-        const uint32_t t_hi_a = c_lo_a + K::C_BYTES, t_lo_a = t_hi_a + K::T_BYTES;
-        // ---- GEMM1: S = R C^T, three tf32 products, the small ones first ----
-        wg_fence();
+    int it = 0;
+    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const int rt = u / n_split, sp = u % n_split;
+        const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
+        const int64_t row_a = (int64_t)rt * BM + 64 * cw + 16 * w + g;        // this thread's rows: row_a, row_a + 8
+        // GEMM1's A operand, read once per unit straight into the tf32 A fragment (same layout as GEMM2's, see exp_tile):
+        // r[4kk + 2c + h] = R(row_a + 8h, 8kk + t + 4c); rows past n_r are 0
 #pragma unroll
-        for (int part = 0; part < 3; ++part) {
-            const uint32_t ra = (part == 0) ? r_lo_a : r_hi_a;
-            const uint32_t cb = (part == 1) ? c_lo_a : c_hi_a;
+        for (int h = 0; h < 2; ++h) {
+            const int64_t row = row_a + 8 * h;
+            const bool ok = row < n_r;
 #pragma unroll
-            for (int kk = 0; kk < D / 8; ++kk) {
-                const uint32_t koff = (kk & 3) * 32;
-                wgmma_ss_n64(sacc, wg_desc(ra + (kk >> 2) * K::R_CHUNK + koff), wg_desc(cb + (kk >> 2) * K::C_CHUNK + koff),
-                             (part > 0 || kk > 0) ? 1u : 0u);
-            }
+            for (int kk = 0; kk < D / 8; ++kk)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int64_t at = row * D + 8 * kk + t + 4 * c;
+                    rhi[4 * kk + 2 * c + h] = ok ? __float_as_uint(__ldg(R_hi + at)) : 0u;
+                    rlo[4 * kk + 2 * c + h] = ok ? __float_as_uint(__ldg(R_lo + at)) : 0u;
+                }
         }
-        wg_commit();
-        wg_wait0();
-        reg_fence(sacc);
-        // ---- E = exp2(S - offset) * colscale, row sums, GEMM2's A fragment ----
-        const int64_t col0 = (int64_t)(t0 + i) * BN;
-        if (col0 + BN <= n_c) exp_tile<false>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
-        else exp_tile<true>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
-        // ---- GEMM2: O += E C (hi*hi into O, the two correction products into OC) ----
-        wg_fence();
 #pragma unroll
-        for (int part = 0; part < 3; ++part) {
-            const uint32_t *ea = (part == 0) ? alo : ahi;
-            const uint32_t tb = (part == 1) ? t_lo_a : t_hi_a;
+        for (int k = 0; k < D / 2; ++k) o[k] = oc[k] = 0.f;
+        float rowsum[2] = {0.f, 0.f};
+        for (int tile = t0; tile < t1; ++tile, ++it) {
+            const int s = it % ST;
+            mbar_wait(&full[s], (it / ST) & 1);
+            const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::C_BYTES;
+            const uint32_t t_hi_a = c_lo_a + K::C_BYTES, t_lo_a = t_hi_a + K::T_BYTES;
+            // ---- GEMM1: S = R C^T, three tf32 products, the small ones first ----
+            named_sync(bar_mine);
+            wg_fence();
 #pragma unroll
-            for (int kk = 0; kk < BN / 8; ++kk) {
-                const uint64_t bd = wg_desc(tb + (kk >> 2) * K::T_CHUNK + (kk & 3) * 32);
-                if (part == 2) wgmma_rs<D>(o, ea + 4 * kk, bd);
-                else wgmma_rs<D>(oc, ea + 4 * kk, bd);
+            for (int part = 0; part < 3; ++part) {
+                const uint32_t *ra = (part == 0) ? rlo : rhi;
+                const uint32_t cb = (part == 1) ? c_lo_a : c_hi_a;
+#pragma unroll
+                for (int kk = 0; kk < D / 8; ++kk)
+                    wgmma_rs_n64(sacc, ra + 4 * kk, wg_desc(cb + (kk >> 2) * K::C_CHUNK + (kk & 3) * 32), (part > 0 || kk > 0) ? 1u : 0u);
             }
+            wg_commit();
+            named_arrive(bar_other);
+            wg_wait0();
+            reg_fence(sacc);
+            reg_fence(rhi);
+            reg_fence(rlo);
+            // ---- E = exp2(S - offset) * colscale, row sums, GEMM2's A fragment ----
+            const int64_t col0 = (int64_t)tile * BN;
+            if (col0 + BN <= n_c) exp_tile<false>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
+            else exp_tile<true>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
+            // ---- GEMM2: O += E C (hi*hi into O, the two correction products into OC) ----
+            named_sync(bar_mine);
+            wg_fence();
+#pragma unroll
+            for (int part = 0; part < 3; ++part) {
+                const uint32_t *ea = (part == 0) ? alo : ahi;
+                const uint32_t tb = (part == 1) ? t_lo_a : t_hi_a;
+#pragma unroll
+                for (int kk = 0; kk < BN / 8; ++kk) {
+                    const uint64_t bd = wg_desc(tb + (kk >> 2) * K::T_CHUNK + (kk & 3) * 32);
+                    if (part == 2) wgmma_rs<D>(o, ea + 4 * kk, bd);
+                    else wgmma_rs<D>(oc, ea + 4 * kk, bd);
+                }
+            }
+            wg_commit();
+            named_arrive(bar_other);
+            // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas
+            wg_wait0();
+            reg_fence(ahi);
+            reg_fence(alo);
+            reg_fence(o);
+            reg_fence(oc);
+            mbar_arrive(&empty[s]);                               // both copies of the tile are consumed
         }
-        wg_commit();
-        // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas; the other
-        // consumer warpgroup's MMAs fill the tensor pipe meanwhile
-        wg_wait0();
-        reg_fence(ahi);
-        reg_fence(alo);
-        reg_fence(o);
-        reg_fence(oc);
-        mbar_arrive(&empty[s]);                               // both copies of tile i are consumed
-    }
 
-    // ---- epilogue: o[4j + 2h + c] = O(row 16w + g + 8h, col 8j + 2t + c) ----
+        // ---- unit epilogue: o[4j + 2h + c] = O(row 16w + g + 8h, col 8j + 2t + c) ----
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
-        rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
-        const int64_t grow = (int64_t)row0 + (wg - 1) * 64 + 16 * w + g + 8 * h;
-        if (grow >= n_r) continue;
-        float *dst = o_part + ((size_t)sp * n_r + grow) * D;
+        for (int h = 0; h < 2; ++h) {
+            rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
+            rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
+            const int64_t grow = row_a + 8 * h;
+            if (grow >= n_r) continue;
+            float *dst = o_part + ((size_t)sp * n_r + grow) * D;
 #pragma unroll
-        for (int j = 0; j < D / 8; ++j)
-            *reinterpret_cast<float2 *>(dst + 8 * j + 2 * t) =
-                make_float2(o[4 * j + 2 * h] + oc[4 * j + 2 * h], o[4 * j + 2 * h + 1] + oc[4 * j + 2 * h + 1]);
-        if (t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h];
+            for (int j = 0; j < D / 8; ++j)
+                *reinterpret_cast<float2 *>(dst + 8 * j + 2 * t) =
+                    make_float2(o[4 * j + 2 * h] + oc[4 * j + 2 * h], o[4 * j + 2 * h + 1] + oc[4 * j + 2 * h + 1]);
+            if (t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h];
+        }
     }
+    if (cw == 0) named_sync(1);                                  // consumer 1's last hand-over
 }
 
 // ---- host side: tensor maps through the driver entry point (no link-time libcuda dependency) ----
@@ -374,25 +398,34 @@ template <int D>
 int launch_tc(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo, const float *CT_hi,
               const float *CT_lo, int64_t ct_pitch, int64_t n_c, const float *colscale, float offset, int n_split,
               float *rowsum_part, float *o_part, cudaStream_t st) {
-    CUtensorMap mr_hi, mr_lo, mc_hi, mc_lo, mt_hi, mt_lo;
+    CUtensorMap mc_hi, mc_lo, mt_hi, mt_lo;
     int rc;
-    if ((rc = make_map(&mr_hi, R_hi, n_r, D, D, BM)) != SSL_OK) return rc;
-    if ((rc = make_map(&mr_lo, R_lo, n_r, D, D, BM)) != SSL_OK) return rc;
     if ((rc = make_map(&mc_hi, C_hi, n_c, D, D, BN)) != SSL_OK) return rc;
     if ((rc = make_map(&mc_lo, C_lo, n_c, D, D, BN)) != SSL_OK) return rc;
-    if ((rc = make_map(&mt_hi, CT_hi, D, n_c, ct_pitch, D)) != SSL_OK) return rc;
-    if ((rc = make_map(&mt_lo, CT_lo, D, n_c, ct_pitch, D)) != SSL_OK) return rc;
+    // the transposed copy's columns are permuted within groups of 8 (see exp_tile): its last group is read whole
+    const int64_t n_c8 = (n_c + 7) / 8 * 8;
+    if ((rc = make_map(&mt_hi, CT_hi, D, n_c8, ct_pitch, D)) != SSL_OK) return rc;
+    if ((rc = make_map(&mt_lo, CT_lo, D, n_c8, ct_pitch, D)) != SSL_OK) return rc;
     const size_t smem = Cfg<D>::SMEM;
-    // cudaFuncSetAttribute is per DEVICE: remember which devices of this process are configured
+    // cudaFuncSetAttribute is per DEVICE: remember which devices of this process are configured, and their SM counts
     static bool configured[64] = {};
-    int dev = 0;
+    static int sm_count[64] = {};
+    int dev = 0, n_sm = 0;
     SSL_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
+    if (dev >= 0 && dev < 64 && configured[dev]) {
+        n_sm = sm_count[dev];
+    } else {
         SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < 64) configured[dev] = true;
+        SSL_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+        if (dev >= 0 && dev < 64) {
+            sm_count[dev] = n_sm;
+            configured[dev] = true;
+        }
     }
-    const int64_t grid = ((n_r + BM - 1) / BM) * n_split;
-    softmax_gemm_tc_kernel<D><<<(unsigned)grid, kNumThreads, smem, st>>>(mr_hi, mr_lo, mc_hi, mc_lo, mt_hi, mt_lo, n_r, n_c, colscale, offset,
+    // persistent: one CTA per SM, each looping over units (R tile, C chunk) blockIdx.x, + gridDim.x, ...
+    const int64_t units = ((n_r + BM - 1) / BM) * n_split;
+    const int64_t grid = units < n_sm ? units : n_sm;
+    softmax_gemm_tc_kernel<D><<<(unsigned)grid, kNumThreads, smem, st>>>(R_hi, R_lo, mc_hi, mc_lo, mt_hi, mt_lo, n_r, n_c, colscale, offset,
                                                                          n_split, rowsum_part, o_part);
     SSL_LAUNCH_CHECK("softmax_gemm_tc_kernel");
     return SSL_OK;
@@ -405,7 +438,7 @@ extern "C" int ssl_softmax_gemm_tf32x3(const float *R_hi, const float *R_lo, int
                                        const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                                        void *stream) {
     SSL_CHECK_ARG(R_hi && R_lo && C_hi && C_lo && CT_hi && CT_lo && o_part, "ssl_softmax_gemm_tf32x3: null argument");
-    SSL_CHECK_ARG(ct_pitch >= n_c && ct_pitch % 4 == 0, "ssl_softmax_gemm_tf32x3: ct_pitch must be >= n_c and a multiple of 4");
+    SSL_CHECK_ARG(ct_pitch >= (n_c + 7) / 8 * 8 && ct_pitch % 4 == 0, "ssl_softmax_gemm_tf32x3: ct_pitch must be >= ceil8(n_c) and a multiple of 4");
     SSL_CHECK_ARG(dim == 32 || dim == 64, "ssl_softmax_gemm_tf32x3: dim %d not supported (32 or 64; other sizes use ssl_softmax_gemm)", dim);
     SSL_CHECK_ARG((n_split >= 1 && n_split <= (n_c + BN - 1) / BN) || n_c == 0, "ssl_softmax_gemm_tf32x3: n_split %d exceeds the number of C tiles", n_split);
     SSL_CHECK_ARG(((reinterpret_cast<uintptr_t>(R_hi) | reinterpret_cast<uintptr_t>(R_lo) | reinterpret_cast<uintptr_t>(C_hi) |

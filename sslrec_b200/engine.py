@@ -691,16 +691,17 @@ def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_f
     """Number of chunks the streamed operand is cut into: n_rtiles * n_split CTAs on ``slots`` resident-CTA slots (2 per SM for
     the FFMA kernel at dim <= 64, 1 per SM for the tensor-core kernel), every CTA keeping >= 4 tiles.
 
-    ``prefer_few`` (the tensor-core kernel): minimise  waves(s) * (tiles_per_cta(s) + c)  with c = 5.5 tile-times of per-CTA
-    overhead (resident-tile load, pipeline fill, O write-out); fewer, longer CTAs than the pure wave-efficiency rule picks.
-    c was fitted to the contraction kernel this wgmma kernel replaced and has not been re-measured for it (a sweep:
-    tools/perf_tc.py sweep); the split only changes how the work is cut, never the result beyond summation order.
+    ``prefer_few`` (the persistent tensor-core kernel, one CTA per SM looping over n_rtiles * n_split units): minimise
+    rounds(s) * (tiles_per_unit(s) + c)  with c = 5 tile-times of per-unit overhead (R fragment load, pipeline restart,
+    O write-out), fitted to an n_split sweep of that kernel at the amazon forward shape on an H100 (profiles/r04_nce_tc.md);
+    fewer, longer units than the pure wave-efficiency rule picks.  The split only changes how the work is cut, never the
+    result beyond summation order.
     Otherwise: the split with the best wave efficiency (FFMA kernel)."""
     max_split = max(1, min(n_ctiles // 4 if n_ctiles >= 4 else 1, 64))
     if prefer_few:
         best, best_cost = 1, None
         for s in range(1, max_split + 1):
-            cost = math.ceil(n_rtiles * s / slots) * (math.ceil(n_ctiles / s) + 5.5)
+            cost = math.ceil(n_rtiles * s / slots) * (math.ceil(n_ctiles / s) + 5.0)
             if best_cost is None or cost < best_cost - 1e-9:
                 best, best_cost = s, cost
         return best
