@@ -29,7 +29,7 @@ def _plan(adj, need_rev=False):
     return GraphPlan(adj.rows, adj.cols, adj.vals, adj.n, torch.device('cuda'), need_rev=need_rev)
 
 
-@pytest.mark.parametrize('dim', [16, 32, 64, 128, 48])
+@pytest.mark.parametrize('dim', [16, 32, 64, 128, 48, 4, 20, 68, 124])
 @pytest.mark.parametrize('hub', [0, 700])
 def test_propagation_matches_oracle(dim, hub):
     from sslrec_b200 import engine as E
@@ -49,15 +49,35 @@ def test_propagation_matches_oracle(dim, hub):
 
 
 def test_three_views_share_layer_one_and_match_single_views():
+    """A V-view propagation (3 layers, layer sum) equals V one-view propagations of its views, bit for bit: the three SimGCL
+    views (two noisy, one clean) and in general V = 2..4 views at every lane-group dim, with per-view noise (MODE 0 at layer 1,
+    MODE 1 after) or mixed per-view edge modes (MODE 2), through the interleaved and the view-major kernel.  The hub row has
+    4097 entries: 256-entry segments."""
     from sslrec_b200 import engine as E
-    adj = _graph(500, 400, 5000, 6, 300)
+    from sslrec_b200._lib import check, lib
+    adj = _graph(5000, 400, 20000, 6, 4097)
     plan = _plan(adj)
-    e0 = (torch.randn(adj.n, 64, generator=torch.Generator().manual_seed(2)) * 0.1).cuda()
-    views = [E.ViewSpec(noise_mode=1, seed=11), E.ViewSpec(noise_mode=1, seed=12), E.ViewSpec()]
-    st3 = E.Propagation(plan, views, 3, noise_eps=0.2).forward(e0, 500)
-    for v, spec in enumerate(views):
-        st1 = E.Propagation(plan, [spec], 3, noise_eps=0.2).forward(e0, 500)
-        assert torch.equal(st3.E[:, v, :], st1.E[:, 0, :])
+    assert plan.stats()['max_row_nnz'] == 4097
+    g = torch.Generator().manual_seed(2)
+    mask = (torch.rand(adj.nnz, generator=g) < 0.5).to(torch.uint8).cuda()
+    for dim in (4, 12, 16, 20, 32, 36, 48, 64, 68, 124, 128):
+        e0 = (torch.randn(adj.n, dim, generator=g) * 0.1).cuda()
+        u = [torch.rand(adj.n, dim, generator=g).cuda() for _ in range(3)]
+        noisy = [E.ViewSpec(noise_mode=1, seed=11), E.ViewSpec(noise_mode=1, seed=12), E.ViewSpec(), E.ViewSpec(noise_mode=2, noise_u=u)]
+        masked = [E.ViewSpec(edge_mode=1, keep=0.5, scale=2.0, seed=13), E.ViewSpec(noise_mode=1, seed=14),
+                  E.ViewSpec(edge_mode=2, keep=0.5, scale=2.0, edge_masks=mask), E.ViewSpec(edge_mode=1, keep=0.8, scale=1.25, seed=15)]
+        run = lambda views: E.Propagation(plan, views, 3, noise_eps=0.2).forward(e0, 5000).E
+        for views in (noisy, masked):
+            for V in (2, 3, 4):
+                packed = run(views[:V])
+                check(lib.ssl_set_option(b'prop_view_major', 1), 'ssl_set_option')
+                try:
+                    vm = run(views[:V])
+                finally:
+                    check(lib.ssl_set_option(b'prop_view_major', 0), 'ssl_set_option')
+                assert torch.equal(vm, packed), (dim, V, 'view-major')
+                for v in range(V):
+                    assert torch.equal(run([views[v]])[:, 0], packed[:, v]), (dim, V, v)
 
 
 def test_injected_noise_matches_oracle_and_rng_noise_has_norm_eps():
