@@ -311,12 +311,16 @@ SSL_API int ssl_topk(const float *preds, int64_t n_b, int64_t n_item, int32_t k,
  * uniformity(x) = log mean_{i<j} exp(-2 |x^_i - x^_j|^2): the pair sum is ssl_softmax_gemm[_tf32x3]
  *   with R = 4 log2(e) x^, C = x^, offset = 4 log2(e); ssl_uniform_finalize reduces its split partials
  *   and removes the i == j term: pair_sum[i] = sum_{j!=i} e_ij, w[i,:] = sum_{j!=i} e_ij x^_j.
+ * ssl_uniform_pairs: the same pair_sum / w computed directly, e_ij = exp(-2 |x^_i - x^_j|^2) from the
+ *   difference vector over j != i, one warp per row, O(B^2 d).  Used below 256 rows, where rowsum_i - e_ii
+ *   above loses most of its digits to cancellation.
  * ssl_unit_rows_bwd: dx^_b = scale * (*gscale) * (c1 d1_b + c2 d2_b) pushed through the normalisation,
  *   g_out[idx[b]] += rinv_b (dx^_b - x^_b (x^_b . dx^_b))   (d2 may be NULL; idx NULL = identity).
  * ------------------------------------------------------------------------------------------ */
 SSL_API int ssl_align_fwd(const float *xhat, const float *yhat, int64_t batch, int32_t dim, float *loss_b, void *stream);
 SSL_API int ssl_uniform_finalize(const float *rowsum_part, const float *o_part, int32_t n_split, int64_t batch, int32_t dim,
                          const float *r_scaled, const float *xhat, float offset, float *pair_sum, float *w, void *stream);
+SSL_API int ssl_uniform_pairs(const float *xhat, int64_t batch, int32_t dim, float *pair_sum, float *w, void *stream);
 SSL_API int ssl_unit_rows_bwd(const float *xhat, const float *rinv, const int64_t *idx, int64_t batch, int32_t dim, const float *d1,
                       float c1, const float *d2, float c2, const float *gscale, float scale, float *g_out, int64_t g_stride,
                       void *stream);

@@ -90,6 +90,7 @@ def _load():
         'ssl_spmm_exact': (C.c_int, [vp, vp, vp, i64, vp, i64, i32, vp, i64, vp]),
         'ssl_align_fwd': (C.c_int, [vp, vp, i64, i32, vp, vp]),
         'ssl_uniform_finalize': (C.c_int, [vp, vp, i32, i64, i32, vp, vp, f32, vp, vp, vp]),
+        'ssl_uniform_pairs': (C.c_int, [vp, i64, i32, vp, vp, vp]),
         'ssl_unit_rows_bwd': (C.c_int, [vp, vp, vp, i64, i32, vp, f32, vp, f32, vp, f32, vp, i64, vp]),
         'ssl_kmeans_workspace': (C.c_int, [i64, i32, i32, c_i32p, c_i32p]),
         'ssl_kmeans_iter': (C.c_int, [vp, i64, i64, i32, i32, vp, vp, vp, vp, vp, vp, vp]),

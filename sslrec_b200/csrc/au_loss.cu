@@ -1,8 +1,8 @@
 // DirectAU's alignment / uniformity losses (models/loss_utils.py:75-86) on unit rows produced by
 // ssl_rows_normalize(norm_mode 2 = F.normalize).  The B x B pair sum of the uniformity term is the
 // softmax contraction of nce_gemm*.cu with R = C = x^ (e_ij = exp(4 x^_i.x^_j - 4) = exp(-2 |x^_i - x^_j|^2));
-// the kernels here are its epilogue, the row-wise alignment term and the shared backward through
-// the normalisation.  One warp per row, lanes over the dim.
+// the kernels here are its epilogue, the direct pair sum used below 256 rows, the row-wise alignment
+// term and the shared backward through the normalisation.  One warp per row, lanes over the dim.
 #include "common.cuh"
 
 namespace {
@@ -68,6 +68,34 @@ __global__ void uniform_finalize_kernel(const float *rowsum_part, const float *o
     if (lane == 0) pair_sum[b] = rs - e_ii;
 }
 
+// Direct pair sums for small batches: the same pair_sum / w as uniform_finalize_kernel, but e_ij = exp(-2 |x^_i - x^_j|^2)
+// from the difference vector over j != i in increasing order, as pdist does.  rowsum - e_ii cancels when the off-diagonal
+// sum is small next to e_ii = 1 (B = 2-3, near-antipodal rows); this form has no such cancellation.  O(B^2 d) work.
+__global__ void uniform_pairs_kernel(const float *xhat, int64_t batch, int dim, float *pair_sum, float *w) {
+    const int lane = threadIdx.x & 31;
+    const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (b >= batch) return;
+    float x[kMaxPerLane], y[kMaxPerLane], df[kMaxPerLane], o[kMaxPerLane] = {0.f, 0.f, 0.f, 0.f};
+    load_row(xhat + b * dim, dim, lane, x);
+    float ps = 0.f;
+    for (int64_t j = 0; j < batch; ++j) {
+        if (j == b) continue;
+        load_row(xhat + j * dim, dim, lane, y);
+#pragma unroll
+        for (int i = 0; i < kMaxPerLane; ++i) df[i] = x[i] - y[i];
+        const float e = expf(-2.f * dot_rows(df, df));
+        ps += e;
+#pragma unroll
+        for (int i = 0; i < kMaxPerLane; ++i) o[i] = fmaf(e, y[i], o[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < kMaxPerLane; ++i) {
+        const int k = lane + 32 * i;
+        if (k < dim) w[b * dim + k] = o[i];
+    }
+    if (lane == 0) pair_sum[b] = ps;
+}
+
 // dx^_b = g (c1 d1_b + c2 d2_b), g = scale * (*gscale); through x^ = x * rinv:
 // de_b = rinv_b (dx^_b - x^_b (x^_b . dx^_b)), added to row idx[b] of the gradient view.
 __global__ void unit_rows_bwd_kernel(const float *xhat, const float *rinv, const int64_t *idx, int64_t batch, int dim,
@@ -118,6 +146,15 @@ extern "C" int ssl_uniform_finalize(const float *rowsum_part, const float *o_par
     uniform_finalize_kernel<<<(unsigned)((batch + 7) / 8), 256, 0, STREAM>>>(rowsum_part, o_part, n_split, batch, dim, r_scaled, xhat,
                                                                              offset, pair_sum, w);
     SSL_LAUNCH_CHECK("uniform_finalize_kernel");
+    return SSL_OK;
+}
+
+extern "C" int ssl_uniform_pairs(const float *xhat, int64_t batch, int32_t dim, float *pair_sum, float *w, void *stream) {
+    SSL_CHECK_ARG(xhat && pair_sum && w, "ssl_uniform_pairs: null argument");
+    SSL_CHECK_ARG(dim >= 1 && dim <= SSL_MAX_DIM, "ssl_uniform_pairs: bad dim");
+    if (batch == 0) return SSL_OK;
+    uniform_pairs_kernel<<<(unsigned)((batch + 7) / 8), 256, 0, STREAM>>>(xhat, batch, dim, pair_sum, w);
+    SSL_LAUNCH_CHECK("uniform_pairs_kernel");
     return SSL_OK;
 }
 

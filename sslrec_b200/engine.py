@@ -971,22 +971,31 @@ def _align_bwd(pack, g):
 
 
 def _uniform_fwd(x: Rows, ix):
-    """uniformity(x) = log mean_{i<j} exp(-2 |x^_i - x^_j|^2) (loss_utils.py:82-86): the B x B pair sum runs on the
-    InfoNCE contraction kernel (R = 4 log2e x^, C = x^), never materialising pdist's B(B-1)/2 vector."""
+    """uniformity(x) = log mean_{i<j} exp(-2 |x^_i - x^_j|^2) (loss_utils.py:82-86): from 256 rows on, the B x B pair sum
+    runs on the InfoNCE contraction kernel (R = 4 log2e x^, C = x^), never materialising pdist's B(B-1)/2 vector."""
     dev, d, B = x.base.device, x.dim, ix.numel()
     if B < 2:
         raise ValueError('uniformity needs at least 2 rows')
+    f = dict(device=dev, dtype=torch.float32)
+    pair_sum, w, total = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty((), **f)
+    if B < 256:
+        # The contraction's pair_sum_i = rowsum_i - e_ii cancels when the off-diagonal sum is small next to e_ii = 1
+        # (B = 2-3, near-antipodal rows).  Below 256 rows the pairs are summed directly from x^_i - x^_j instead.
+        c, rinv, _ = _unit_rows(x, ix, 1.0, False, False)
+        with torch.cuda.device(dev):
+            s = _stream(x.base)
+            check(lib.ssl_uniform_pairs(c.data_ptr(), B, d, pair_sum.data_ptr(), w.data_ptr(), s), 'ssl_uniform_pairs')
+            check(lib.ssl_sum(pair_sum.data_ptr(), B, 1.0, total.data_ptr(), s), 'ssl_sum')
+        out = torch.log(total / float(B * (B - 1)))
+        return out, (x, ix, c, rinv, w, total)
     Bp = ceil_to(B, 64)
-    # pair_sum_i = rowsum_i - e_ii cancels when the batch is tiny (e_ii = 1 against a handful of e_ij ~ 1e-2): there the
-    # FP32-FMA contraction (1e-7 relative) is used, the 3xTF32 one (1e-6) from 256 rows on, where the pair sum is >> e_ii
-    use_tc = USE_TENSOR_CORES and d in (32, 64) and B >= 256
+    # from 256 rows on the pair sum is >> e_ii, so removing e_ii loses little and the 3xTF32 contraction (1e-6) suffices
+    use_tc = USE_TENSOR_CORES and d in (32, 64)
     off = 4.0 * LOG2E
     r, _, (r_hi, r_lo, _, _, _) = _unit_rows(x, ix, off, False, use_tc)
     c, rinv, (c_hi, c_lo, c_thi, c_tlo, c_t) = _unit_rows(x, ix, 1.0, True, use_tc)
-    f = dict(device=dev, dtype=torch.float32)
     n_split = choose_split((B + 127) // 128, Bp // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
     rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
-    pair_sum, w, total = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty((), **f)
     with torch.cuda.device(dev):
         s = _stream(x.base)
         with _timed('nce_gemm_fwd', dict(B=B, n=B, dim=d, tc=use_tc)):
