@@ -257,6 +257,59 @@ SSL_API int ssl_lse_finalize(const float *rowsum_part, const float *o_part, int3
 SSL_API int ssl_nce_colscale(const float *rowsum, int64_t batch, const float *gscale, float scale, float *colscale, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * a13b  the InfoNCE pieces bounded by a DEVICE row count: a term over a padded anchor list whose
+ * live length only the device knows (HCCF's spec-node term under CUDA-graph capture, fed by
+ * ssl_unique_ids).  n_live points to an int64 on the device, clamped to [0, capacity]; the host
+ * passes the capacity, so buffer shapes, tensor maps and n_split depend on host-known sizes only.
+ *
+ * ssl_softmax_gemm_live / ssl_softmax_gemm_tf32x3_live: the contractions above, with
+ *   live_role SSL_LIVE_ROWS: only rows r < *n_live of R are live (the forward, R = anchors).  Their
+ *     outputs equal those of the plain call at n_r = *n_live bit for bit; rows >= *n_live of
+ *     o_part / rowsum_part are not written (the row pitch stays n_r).  Units whose R tile starts
+ *     at or past the count are skipped.
+ *   live_role SSL_LIVE_COLS: only rows c < *n_live of C are live (the backward, C = anchors).
+ *     The chunks are cut from the live tile count, columns past it are masked (colscale there is
+ *     never read), and a chunk left empty writes zero partials.  Outputs equal the plain call at
+ *     n_c = *n_live bit for bit, for every n_split that call accepts; C rows past the count must
+ *     be finite.
+ * ssl_sum_live: out[0] = alpha / live * sum_{b < live} x[b]  (0 when live = 0).
+ * ssl_nce_bwd_rows_live: ssl_nce_bwd_rows over the rows b < live only, with g = scale / live * (*gscale).
+ * ssl_nce_colscale_live: colscale[b] = scale / live * (*gscale) * ln2 / rowsum[b] for b < live, 0 past it.
+ * ------------------------------------------------------------------------------------------ */
+#define SSL_LIVE_ROWS 1
+#define SSL_LIVE_COLS 2
+SSL_API int ssl_softmax_gemm_live(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int32_t dim,
+                          const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
+                          const int64_t *n_live, int32_t live_role, void *stream);
+SSL_API int ssl_softmax_gemm_tf32x3_live(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo,
+                                 const float *CT_hi, const float *CT_lo, int64_t ct_pitch, int64_t n_c, int32_t dim,
+                                 const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
+                                 const int64_t *n_live, int32_t live_role, void *stream);
+SSL_API int ssl_sum_live(const float *x, int64_t n, const int64_t *n_live, float alpha, float *out, void *stream);
+SSL_API int ssl_nce_bwd_rows_live(const float *a_hat, const float *p_hat, const float *obar, const float *rinv1, const float *rinv2,
+                          const int64_t *idx, int64_t batch, const int64_t *n_live, int32_t dim, float tau, const float *gscale,
+                          float scale, float *g1, int64_t g1_stride, float *g2, int64_t g2_stride, void *stream);
+SSL_API int ssl_nce_colscale_live(const float *rowsum, int64_t batch, const int64_t *n_live, const float *gscale, float scale,
+                          float *colscale, void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * a13c  ssl_unique_ids: sorted de-duplication on the device, the graph-safe form of HCCF's
+ * t.unique(ancs) / t.unique(poss) (hccf.py:80-81 of the reference).
+ *   idx [n] int64, every id in [0, n_range) (a precondition; ids outside are not counted).
+ *   out [n] int64: out[0, *count) = the distinct ids ascending (torch.unique(idx, sorted=True));
+ *     out[*count, n) repeat the largest id, so a gather through the whole padded list stays in bounds.
+ *   count: an int64 on the DEVICE.
+ *   scratch: caller-owned, 16-byte aligned, scratch_n_words uint32 words (ssl_unique_ids_scratch):
+ *     a bitmap of ceil(n_range / 32) words padded to whole 1024-word blocks, plus the block sums.
+ *     The launch sequence clears it itself, so a CUDA-graph replay with new indices is correct.
+ * Five launches (clear, mark, per-block popcount, scan, compact + padding); O(n + n_range / 32);
+ * the result does not depend on scheduling.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_unique_ids_scratch(int64_t n_range, int64_t *words);
+SSL_API int ssl_unique_ids(const int64_t *idx, int64_t n, int64_t n_range, uint32_t *scratch, int64_t scratch_n_words,
+                   int64_t *out, int64_t *count, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * a15  reg_params (loss_utils.py:20-24): out[0] = sum x^2, deterministic two-stage reduction.
  * ssl_sum: out[0] = alpha * sum x (same reduction; used for the per-sample loss vectors).
  * ssl_axpy: y += alpha * (*gscale) * x  (gradient of the regulariser, 2 * reg_weight * W).

@@ -74,6 +74,13 @@ def _load():
         'ssl_nce_bwd_rows': (C.c_int, [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp, f32, vp, i64, vp, i64, vp]),
         'ssl_nce_bwd_table': (C.c_int, [vp, i32, vp, vp, i64, i32, vp, i64, i32, vp]),
         'ssl_nce_colscale': (C.c_int, [vp, i64, vp, f32, vp, vp]),
+        'ssl_softmax_gemm_live': (C.c_int, [vp, i64, vp, vp, i64, i32, vp, f32, i32, vp, vp, vp, i32, vp]),
+        'ssl_softmax_gemm_tf32x3_live': (C.c_int, [vp, vp, i64, vp, vp, vp, vp, i64, i64, i32, vp, f32, i32, vp, vp, vp, i32, vp]),
+        'ssl_sum_live': (C.c_int, [vp, i64, vp, f32, vp, vp]),
+        'ssl_nce_bwd_rows_live': (C.c_int, [vp, vp, vp, vp, vp, vp, i64, vp, i32, f32, vp, f32, vp, i64, vp, i64, vp]),
+        'ssl_nce_colscale_live': (C.c_int, [vp, i64, vp, vp, f32, vp, vp]),
+        'ssl_unique_ids_scratch': (C.c_int, [i64, c_i64p]),
+        'ssl_unique_ids': (C.c_int, [vp, i64, i64, vp, i64, vp, vp, vp]),
         'ssl_sumsq': (C.c_int, [vp, i64, vp, vp]),
         'ssl_sum': (C.c_int, [vp, i64, f32, vp, vp]),
         'ssl_axpy': (C.c_int, [vp, vp, i64, vp, f32, vp]),

@@ -109,6 +109,12 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// the live count of a device-bounded launch (the *_live entry points): *n_live clamped to [0, cap]
+__device__ __forceinline__ int64_t live_count(const int64_t *n_live, int64_t cap) {
+    const int64_t v = *n_live;
+    return v < 0 ? 0 : (v > cap ? cap : v);
+}
+
 __device__ __forceinline__ float4 ldg4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
 __device__ __forceinline__ void fma4(float4 &a, float w, const float4 &x) {
     a.x = fmaf(w, x.x, a.x);

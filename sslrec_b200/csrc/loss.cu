@@ -205,14 +205,30 @@ __global__ void nce_colscale_kernel(const float *rowsum, int64_t batch, const fl
     if (b >= batch) return;
     colscale[b] = scale * (gscale ? __ldg(gscale) : 1.f) * kLn2 / rowsum[b];
 }
+// ssl_nce_colscale_live: the mean over the first `live` anchors; 0 past them, so the swapped gemm sums nothing from a padding row
+__global__ void nce_colscale_live_kernel(const float *rowsum, int64_t batch, const int64_t *n_live, const float *gscale, float scale,
+                                         float *colscale) {
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= batch) return;
+    const int64_t live = ssl::live_count(n_live, batch);
+    colscale[b] = (b < live) ? (scale / (float)live) * (gscale ? __ldg(gscale) : 1.f) * kLn2 / rowsum[b] : 0.f;
+}
 
 // d a^ = g/tau (obar - p^) ; d p^ = -g/tau a^ ; through x^ = x * rinv:  dx = rinv (dx^ - x^ (x^ . dx^))
+// LIVE (ssl_nce_bwd_rows_live): rows past *n_live are skipped and g is divided by the live count
+template <bool LIVE>
 __global__ void nce_bwd_rows_kernel(const float *a_hat, const float *p_hat, const float *obar, const float *rinv1,
                                     const float *rinv2, const int64_t *idx, int64_t batch, int dim, float tau,
-                                    const float *gscale, float scale, float *g1, int64_t g1s, float *g2, int64_t g2s) {
+                                    const float *gscale, float scale, float *g1, int64_t g1s, float *g2, int64_t g2s,
+                                    const int64_t *n_live) {
     const int lane = threadIdx.x & 31;
     const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (b >= batch) return;
+    if (LIVE) {
+        const int64_t live = ssl::live_count(n_live, batch);
+        if (b >= live) return;
+        scale /= (float)live;
+    }
     const float g = scale * (gscale ? __ldg(gscale) : 1.f) / tau;
     const float unscale = tau * kLn2;             // a_hat rows are scaled by log2e / tau
     float a[kMaxPerLane], p[kMaxPerLane], ob[kMaxPerLane];
@@ -301,6 +317,22 @@ __global__ void __launch_bounds__(256) reduce_stage1(const float *__restrict__ x
         float t = 0.f;
         for (int i = 0; i < 8; ++i) t += sh[i];
         part[blockIdx.x] = t;
+    }
+}
+// ssl_sum_live: sum of the first *n_live entries of a vector with room for n, times alpha / live
+__global__ void __launch_bounds__(1024) sum_live_kernel(const float *__restrict__ x, int64_t n, const int64_t *__restrict__ n_live, float alpha,
+                                                        float *__restrict__ out) {
+    __shared__ float sh[32];
+    const int64_t live = ssl::live_count(n_live, n);
+    float s = 0.f;
+    for (int64_t i = threadIdx.x; i < live; i += 1024) s += x[i];
+    s = ssl::warp_sum(s);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+        for (int i = 0; i < 32; ++i) t += sh[i];
+        out[0] = live > 0 ? (alpha / (float)live) * t : 0.f;
     }
 }
 __global__ void __launch_bounds__(1024) reduce_stage2(const float *__restrict__ part, int n, float alpha, float *__restrict__ out) {
@@ -489,6 +521,16 @@ extern "C" int ssl_nce_colscale(const float *rowsum, int64_t batch, const float 
     return SSL_OK;
 }
 
+extern "C" int ssl_nce_colscale_live(const float *rowsum, int64_t batch, const int64_t *n_live, const float *gscale, float scale,
+                                     float *colscale, void *stream) {
+    SSL_CHECK_ARG(rowsum && colscale && n_live, "ssl_nce_colscale_live: null argument");
+    SSL_CHECK_ARG(batch >= 0, "ssl_nce_colscale_live: batch %lld < 0", (long long)batch);
+    if (batch == 0) return SSL_OK;
+    nce_colscale_live_kernel<<<(unsigned)((batch + 255) / 256), 256, 0, STREAM>>>(rowsum, batch, n_live, gscale, scale, colscale);
+    SSL_LAUNCH_CHECK("nce_colscale_live_kernel");
+    return SSL_OK;
+}
+
 extern "C" int ssl_nce_bwd_rows(const float *a_hat, const float *p_hat, const float *obar, const float *rinv1, const float *rinv2,
                                 const int64_t *idx, int64_t batch, int32_t dim, float tau, const float *gscale, float scale,
                                 float *g1, int64_t g1_stride, float *g2, int64_t g2_stride, void *stream) {
@@ -496,7 +538,19 @@ extern "C" int ssl_nce_bwd_rows(const float *a_hat, const float *p_hat, const fl
     SSL_CHECK_ARG((g1 == nullptr || rinv1) && (g2 == nullptr || rinv2), "ssl_nce_bwd_rows: rinv missing");
     SSL_CHECK_ARG(dim >= 1 && dim <= SSL_MAX_DIM && tau > 0.f, "ssl_nce_bwd_rows: bad argument");
     if (batch == 0 || (g1 == nullptr && g2 == nullptr)) return SSL_OK;
-    nce_bwd_rows_kernel<<<(unsigned)((batch + 7) / 8), 256, 0, STREAM>>>(a_hat, p_hat, obar, rinv1, rinv2, idx, batch, dim, tau, gscale, scale, g1, g1_stride, g2, g2_stride);
+    nce_bwd_rows_kernel<false><<<(unsigned)((batch + 7) / 8), 256, 0, STREAM>>>(a_hat, p_hat, obar, rinv1, rinv2, idx, batch, dim, tau, gscale, scale, g1, g1_stride, g2, g2_stride, nullptr);
+    SSL_LAUNCH_CHECK("nce_bwd_rows_kernel");
+    return SSL_OK;
+}
+
+extern "C" int ssl_nce_bwd_rows_live(const float *a_hat, const float *p_hat, const float *obar, const float *rinv1, const float *rinv2,
+                                     const int64_t *idx, int64_t batch, const int64_t *n_live, int32_t dim, float tau, const float *gscale,
+                                     float scale, float *g1, int64_t g1_stride, float *g2, int64_t g2_stride, void *stream) {
+    SSL_CHECK_ARG(a_hat && p_hat && obar && idx && n_live, "ssl_nce_bwd_rows_live: null argument");
+    SSL_CHECK_ARG((g1 == nullptr || rinv1) && (g2 == nullptr || rinv2), "ssl_nce_bwd_rows_live: rinv missing");
+    SSL_CHECK_ARG(dim >= 1 && dim <= SSL_MAX_DIM && tau > 0.f && batch >= 0, "ssl_nce_bwd_rows_live: bad argument");
+    if (batch == 0 || (g1 == nullptr && g2 == nullptr)) return SSL_OK;
+    nce_bwd_rows_kernel<true><<<(unsigned)((batch + 7) / 8), 256, 0, STREAM>>>(a_hat, p_hat, obar, rinv1, rinv2, idx, batch, dim, tau, gscale, scale, g1, g1_stride, g2, g2_stride, n_live);
     SSL_LAUNCH_CHECK("nce_bwd_rows_kernel");
     return SSL_OK;
 }
@@ -541,6 +595,13 @@ int reduce_impl(const float *x, int64_t n, float alpha, float *out, cudaStream_t
 
 extern "C" int ssl_sumsq(const float *x, int64_t n, float *out, void *stream) { return reduce_impl<true>(x, n, 1.f, out, STREAM, "ssl_sumsq"); }
 extern "C" int ssl_sum(const float *x, int64_t n, float alpha, float *out, void *stream) { return reduce_impl<false>(x, n, alpha, out, STREAM, "ssl_sum"); }
+extern "C" int ssl_sum_live(const float *x, int64_t n, const int64_t *n_live, float alpha, float *out, void *stream) {
+    SSL_CHECK_ARG(x && n_live && out, "ssl_sum_live: null argument");
+    SSL_CHECK_ARG(n >= 0, "ssl_sum_live: n %lld < 0", (long long)n);
+    sum_live_kernel<<<1, 1024, 0, STREAM>>>(x, n, n_live, alpha, out);
+    SSL_LAUNCH_CHECK("sum_live_kernel");
+    return SSL_OK;
+}
 
 extern "C" int ssl_axpy(const float *x, float *y, int64_t n, const float *gscale, float alpha, void *stream) {
     SSL_CHECK_ARG(x && y, "ssl_axpy: null argument");

@@ -58,12 +58,17 @@ __device__ __forceinline__ float ex2(float x) {
     return y;
 }
 
-template <int D>
+// LIVE selects a device-side bound (ssl_softmax_gemm_live): 0 none (n_live unused), 1 only the first min(*n_live, n_r) rows of R
+// are live, 2 only the first min(*n_live, n_c) rows of C.  n_r stays the row pitch of the outputs.
+template <int D, int LIVE>
 __global__ void __launch_bounds__(256, (D <= 64) ? 2 : 1)
 softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__restrict__ C, const float *__restrict__ C_t,
-                    int64_t n_c, int dim, const float *__restrict__ colscale, float offset, int n_split,
-                    float *__restrict__ rowsum_part, float *__restrict__ o_part) {
+                    int64_t n_c_cap, int dim, const float *__restrict__ colscale, float offset, int n_split,
+                    float *__restrict__ rowsum_part, float *__restrict__ o_part, const int64_t *__restrict__ n_live) {
     constexpr int CPT = D / 16;
+    // live extents: rows of R past n_r_live are neither read nor written; columns past n_c are masked like a ragged tail
+    const int64_t n_r_live = (LIVE == 1) ? ssl::live_count(n_live, n_r) : n_r;
+    const int64_t n_c = (LIVE == 2) ? ssl::live_count(n_live, n_c_cap) : n_c_cap;
     extern __shared__ __align__(128) float smem[];
     float *Rs_T = smem;                 // [D][BM]
     float *Cs_T = Rs_T + D * BM;        // [D][BN]   K-major, permuted columns
@@ -76,6 +81,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
     const int64_t n_ct = (n_c + BN - 1) / BN;
     const int64_t t0 = n_ct * sp / n_split, t1 = n_ct * (sp + 1) / n_split;
     const int64_t row0 = (int64_t)rt * BM;
+    if (LIVE == 1 && row0 >= n_r_live) return;         // an R tile wholly past the live rows: nothing to compute or write
 
     for (int i = tid; i < D * BM + D * BN + BN * D; i += 256) smem[i] = 0.f;
     if (tid == 0) {
@@ -97,7 +103,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         const int quads = dim >> 2;
         for (int i = tid; i < BM * quads; i += 256) {
             const int r = i / quads, q = i % quads;
-            if (row0 + r < n_r) {
+            if (row0 + r < n_r_live) {
                 const float4 v = ssl::ldg4(R + (row0 + r) * dim + q * 4);
                 Rs_T[(q * 4 + 0) * BM + r] = v.x;
                 Rs_T[(q * 4 + 1) * BM + r] = v.y;
@@ -200,7 +206,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         v += __shfl_xor_sync(0xffffffffu, v, 2);
         v += __shfl_xor_sync(0xffffffffu, v, 1);
         const int64_t row = row0 + ty * 8 + i;
-        if (row < n_r) {
+        if (row < n_r_live) {
             if (tx == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + row] = v;
             float *dst = o_part + ((size_t)sp * n_r + row) * dim + tx * CPT;
 #pragma unroll
@@ -210,36 +216,63 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
     }
 }
 
-template <int D>
+template <int D, int LIVE>
 int launch(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int dim, const float *colscale,
-           float offset, int n_split, float *rowsum_part, float *o_part, cudaStream_t st) {
+           float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live, cudaStream_t st) {
     const size_t smem = sizeof(float) * (D * BM + D * BN + BN * D + BN * EPITCH) + 2 * sizeof(uint64_t);
     static bool configured[64] = {};      // cudaFuncSetAttribute is per device
     int dev = 0;
     SSL_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !configured[dev]) {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_kernel<D, LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
     const int64_t grid = ((n_r + BM - 1) / BM) * n_split;
-    softmax_gemm_kernel<D><<<(unsigned)grid, 256, smem, st>>>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part);
+    softmax_gemm_kernel<D, LIVE><<<(unsigned)grid, 256, smem, st>>>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part,
+                                                                    o_part, n_live);
     SSL_LAUNCH_CHECK("softmax_gemm_kernel");
     return SSL_OK;
 }
 
 }  // namespace
 
+namespace {
+int check_args(const float *R, const float *C, const float *C_t, int64_t n_c, int32_t dim, int32_t n_split, const float *o_part,
+               const char *name) {
+    SSL_CHECK_ARG(R && C && C_t && o_part, "%s: null argument", name);
+    SSL_CHECK_ARG(dim >= 4 && dim <= SSL_MAX_DIM && dim % 4 == 0, "%s: dim %d must be a multiple of 4 <= %d", name, dim, SSL_MAX_DIM);
+    SSL_CHECK_ARG((n_split >= 1 && n_split <= (n_c + BN - 1) / BN) || n_c == 0, "%s: n_split %d exceeds the number of C tiles", name, n_split);
+    SSL_CHECK_ARG(((reinterpret_cast<uintptr_t>(R) | reinterpret_cast<uintptr_t>(C) | reinterpret_cast<uintptr_t>(C_t)) & 15) == 0,
+                  "%s: operands must be 16-byte aligned", name);
+    return SSL_OK;
+}
+template <int LIVE>
+int dispatch(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int32_t dim, const float *colscale, float offset,
+             int32_t n_split, float *rowsum_part, float *o_part, const int64_t *n_live, cudaStream_t st) {
+    if (dim <= 32) return launch<32, LIVE>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+    if (dim <= 64) return launch<64, LIVE>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+    return launch<128, LIVE>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+}
+}  // namespace
+
 extern "C" int ssl_softmax_gemm(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int32_t dim,
                                 const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                                 void *stream) {
-    SSL_CHECK_ARG(R && C && C_t && o_part, "ssl_softmax_gemm: null argument");
-    SSL_CHECK_ARG(dim >= 4 && dim <= SSL_MAX_DIM && dim % 4 == 0, "ssl_softmax_gemm: dim %d must be a multiple of 4 <= %d", dim, SSL_MAX_DIM);
-    SSL_CHECK_ARG((n_split >= 1 && n_split <= (n_c + BN - 1) / BN) || n_c == 0, "ssl_softmax_gemm: n_split %d exceeds the number of C tiles", n_split);
-    SSL_CHECK_ARG(((reinterpret_cast<uintptr_t>(R) | reinterpret_cast<uintptr_t>(C) | reinterpret_cast<uintptr_t>(C_t)) & 15) == 0,
-                  "ssl_softmax_gemm: operands must be 16-byte aligned");
+    const int rc = check_args(R, C, C_t, n_c, dim, n_split, o_part, "ssl_softmax_gemm");
+    if (rc != SSL_OK) return rc;
     if (n_r == 0 || n_c == 0) return SSL_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dim <= 32) return launch<32>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, st);
-    if (dim <= 64) return launch<64>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, st);
-    return launch<128>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, st);
+    return dispatch<0>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int ssl_softmax_gemm_live(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int32_t dim,
+                                     const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
+                                     const int64_t *n_live, int32_t live_role, void *stream) {
+    const int rc = check_args(R, C, C_t, n_c, dim, n_split, o_part, "ssl_softmax_gemm_live");
+    if (rc != SSL_OK) return rc;
+    SSL_CHECK_ARG(n_live != nullptr, "ssl_softmax_gemm_live: null n_live");
+    SSL_CHECK_ARG(live_role == SSL_LIVE_ROWS || live_role == SSL_LIVE_COLS, "ssl_softmax_gemm_live: bad live_role %d", live_role);
+    if (n_r == 0 || n_c == 0) return SSL_OK;
+    if (live_role == SSL_LIVE_ROWS)
+        return dispatch<1>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, n_live, (cudaStream_t)stream);
+    return dispatch<2>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part, o_part, n_live, (cudaStream_t)stream);
 }

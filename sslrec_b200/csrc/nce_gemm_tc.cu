@@ -190,14 +190,19 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[3
     }
 }
 
-template <int D>
+// LIVE selects a device-side bound (ssl_softmax_gemm_tf32x3_live): 0 none (n_live unused), 1 only the first min(*n_live, n_r)
+// rows of R are live, 2 only the first min(*n_live, n_c) rows of C.  n_r stays the row pitch of the outputs.
+template <int D, int LIVE>
 __global__ void __launch_bounds__(kNumThreads, 1)
 softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__ R_lo,
                        const __grid_constant__ CUtensorMap map_c_hi, const __grid_constant__ CUtensorMap map_c_lo,
                        const __grid_constant__ CUtensorMap map_ct_hi, const __grid_constant__ CUtensorMap map_ct_lo,
-                       int64_t n_r, int64_t n_c, const float *__restrict__ colscale, float offset, int n_split,
-                       float *__restrict__ rowsum_part, float *__restrict__ o_part) {
+                       int64_t n_r, int64_t n_c_cap, const float *__restrict__ colscale, float offset, int n_split,
+                       float *__restrict__ rowsum_part, float *__restrict__ o_part, const int64_t *__restrict__ n_live) {
     using K = Cfg<D>;
+    // live extents: rows of R past n_r_live are neither read nor written; columns past n_c are masked like a ragged tail
+    const int64_t n_r_live = (LIVE == 1) ? ssl::live_count(n_live, n_r) : n_r;
+    const int64_t n_c = (LIVE == 2) ? ssl::live_count(n_live, n_c_cap) : n_c_cap;
     constexpr int ST = K::ST, KCH = K::KCH, JCH = K::JCH;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *ring = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -206,7 +211,7 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
 
     const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
     const int64_t n_ct = (n_c + BN - 1) / BN;
-    const int n_units = (int)((n_r + BM - 1) / BM) * n_split;     // unit u: R tile u / n_split, C chunk u % n_split
+    const int n_units = (int)((n_r_live + BM - 1) / BM) * n_split;     // unit u: R tile u / n_split, C chunk u % n_split
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_hi));
@@ -274,7 +279,7 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int64_t row = row_a + 8 * h;
-            const bool ok = row < n_r;
+            const bool ok = row < n_r_live;
 #pragma unroll
             for (int kk = 0; kk < D / 8; ++kk)
 #pragma unroll
@@ -344,7 +349,7 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
             rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
             rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
             const int64_t grow = row_a + 8 * h;
-            if (grow >= n_r) continue;
+            if (grow >= n_r_live) continue;
             float *dst = o_part + ((size_t)sp * n_r + grow) * D;
 #pragma unroll
             for (int j = 0; j < D / 8; ++j)
@@ -394,10 +399,10 @@ int make_map(CUtensorMap *map, const float *base, int64_t rows, int64_t cols, in
     return SSL_OK;
 }
 
-template <int D>
+template <int D, int LIVE>
 int launch_tc(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo, const float *CT_hi,
               const float *CT_lo, int64_t ct_pitch, int64_t n_c, const float *colscale, float offset, int n_split,
-              float *rowsum_part, float *o_part, cudaStream_t st) {
+              float *rowsum_part, float *o_part, const int64_t *n_live, cudaStream_t st) {
     CUtensorMap mc_hi, mc_lo, mt_hi, mt_lo;
     int rc;
     if ((rc = make_map(&mc_hi, C_hi, n_c, D, D, BN)) != SSL_OK) return rc;
@@ -415,39 +420,68 @@ int launch_tc(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_
     if (dev >= 0 && dev < 64 && configured[dev]) {
         n_sm = sm_count[dev];
     } else {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_tc_kernel<D, LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         SSL_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         if (dev >= 0 && dev < 64) {
             sm_count[dev] = n_sm;
             configured[dev] = true;
         }
     }
-    // persistent: one CTA per SM, each looping over units (R tile, C chunk) blockIdx.x, + gridDim.x, ...
+    // persistent: one CTA per SM, each looping over units (R tile, C chunk) blockIdx.x, + gridDim.x, ...; sized for the
+    // capacity when the live count is on the device (the units past it are skipped, the live ones stay spread round-robin)
     const int64_t units = ((n_r + BM - 1) / BM) * n_split;
     const int64_t grid = units < n_sm ? units : n_sm;
-    softmax_gemm_tc_kernel<D><<<(unsigned)grid, kNumThreads, smem, st>>>(R_hi, R_lo, mc_hi, mc_lo, mt_hi, mt_lo, n_r, n_c, colscale, offset,
-                                                                         n_split, rowsum_part, o_part);
+    softmax_gemm_tc_kernel<D, LIVE><<<(unsigned)grid, kNumThreads, smem, st>>>(R_hi, R_lo, mc_hi, mc_lo, mt_hi, mt_lo, n_r, n_c, colscale,
+                                                                               offset, n_split, rowsum_part, o_part, n_live);
     SSL_LAUNCH_CHECK("softmax_gemm_tc_kernel");
     return SSL_OK;
 }
 
 }  // namespace
 
+namespace {
+int check_tc_args(const float *R_hi, const float *R_lo, const float *C_hi, const float *C_lo, const float *CT_hi, const float *CT_lo,
+                  int64_t ct_pitch, int64_t n_c, int32_t dim, const float *colscale, int32_t n_split, const float *o_part,
+                  const char *name) {
+    SSL_CHECK_ARG(R_hi && R_lo && C_hi && C_lo && CT_hi && CT_lo && o_part, "%s: null argument", name);
+    SSL_CHECK_ARG(ct_pitch >= (n_c + 7) / 8 * 8 && ct_pitch % 4 == 0, "%s: ct_pitch must be >= ceil8(n_c) and a multiple of 4", name);
+    SSL_CHECK_ARG(dim == 32 || dim == 64, "%s: dim %d not supported (32 or 64; other sizes use ssl_softmax_gemm)", name, dim);
+    SSL_CHECK_ARG((n_split >= 1 && n_split <= (n_c + BN - 1) / BN) || n_c == 0, "%s: n_split %d exceeds the number of C tiles", name, n_split);
+    SSL_CHECK_ARG(((reinterpret_cast<uintptr_t>(R_hi) | reinterpret_cast<uintptr_t>(R_lo) | reinterpret_cast<uintptr_t>(C_hi) |
+                    reinterpret_cast<uintptr_t>(C_lo) | reinterpret_cast<uintptr_t>(CT_hi) | reinterpret_cast<uintptr_t>(CT_lo) |
+                    reinterpret_cast<uintptr_t>(o_part)) & 15) == 0,
+                  "%s: operands must be 16-byte aligned", name);
+    SSL_CHECK_ARG((reinterpret_cast<uintptr_t>(colscale) & 7) == 0, "%s: colscale must be 8-byte aligned", name);
+    return SSL_OK;
+}
+}  // namespace
+
 extern "C" int ssl_softmax_gemm_tf32x3(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo,
                                        const float *CT_hi, const float *CT_lo, int64_t ct_pitch, int64_t n_c, int32_t dim,
                                        const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                                        void *stream) {
-    SSL_CHECK_ARG(R_hi && R_lo && C_hi && C_lo && CT_hi && CT_lo && o_part, "ssl_softmax_gemm_tf32x3: null argument");
-    SSL_CHECK_ARG(ct_pitch >= (n_c + 7) / 8 * 8 && ct_pitch % 4 == 0, "ssl_softmax_gemm_tf32x3: ct_pitch must be >= ceil8(n_c) and a multiple of 4");
-    SSL_CHECK_ARG(dim == 32 || dim == 64, "ssl_softmax_gemm_tf32x3: dim %d not supported (32 or 64; other sizes use ssl_softmax_gemm)", dim);
-    SSL_CHECK_ARG((n_split >= 1 && n_split <= (n_c + BN - 1) / BN) || n_c == 0, "ssl_softmax_gemm_tf32x3: n_split %d exceeds the number of C tiles", n_split);
-    SSL_CHECK_ARG(((reinterpret_cast<uintptr_t>(R_hi) | reinterpret_cast<uintptr_t>(R_lo) | reinterpret_cast<uintptr_t>(C_hi) |
-                    reinterpret_cast<uintptr_t>(C_lo) | reinterpret_cast<uintptr_t>(CT_hi) | reinterpret_cast<uintptr_t>(CT_lo) |
-                    reinterpret_cast<uintptr_t>(o_part)) & 15) == 0,
-                  "ssl_softmax_gemm_tf32x3: operands must be 16-byte aligned");
-    SSL_CHECK_ARG((reinterpret_cast<uintptr_t>(colscale) & 7) == 0, "ssl_softmax_gemm_tf32x3: colscale must be 8-byte aligned");
+    const int rc = check_tc_args(R_hi, R_lo, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, dim, colscale, n_split, o_part, "ssl_softmax_gemm_tf32x3");
+    if (rc != SSL_OK) return rc;
     if (n_r == 0 || n_c == 0) return SSL_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    if (dim == 32) return launch_tc<32>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, st);
-    return launch_tc<64>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, st);
+    if (dim == 32) return launch_tc<32, 0>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, nullptr, st);
+    return launch_tc<64, 0>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, nullptr, st);
+}
+
+extern "C" int ssl_softmax_gemm_tf32x3_live(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo,
+                                            const float *CT_hi, const float *CT_lo, int64_t ct_pitch, int64_t n_c, int32_t dim,
+                                            const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
+                                            const int64_t *n_live, int32_t live_role, void *stream) {
+    const int rc = check_tc_args(R_hi, R_lo, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, dim, colscale, n_split, o_part, "ssl_softmax_gemm_tf32x3_live");
+    if (rc != SSL_OK) return rc;
+    SSL_CHECK_ARG(n_live != nullptr, "ssl_softmax_gemm_tf32x3_live: null n_live");
+    SSL_CHECK_ARG(live_role == SSL_LIVE_ROWS || live_role == SSL_LIVE_COLS, "ssl_softmax_gemm_tf32x3_live: bad live_role %d", live_role);
+    if (n_r == 0 || n_c == 0) return SSL_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (live_role == SSL_LIVE_ROWS) {
+        if (dim == 32) return launch_tc<32, 1>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+        return launch_tc<64, 1>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+    }
+    if (dim == 32) return launch_tc<32, 2>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
+    return launch_tc<64, 2>(R_hi, R_lo, n_r, C_hi, C_lo, CT_hi, CT_lo, ct_pitch, n_c, colscale, offset, n_split, rowsum_part, o_part, n_live, st);
 }

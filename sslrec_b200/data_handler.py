@@ -189,13 +189,16 @@ class DeviceTrnData:
             # the flag of datasets_general_cf.py:35-44: 1 on the very first sample served, and on sample 0 once
             # every ``epoch_period`` visits of it
             flags = torch.zeros_like(idx)
+            self.last_flag = False          # whether this batch carries a set flag, known on the host (graphed NCL steps read it)
             if self.epoch_flag_counter == -1:
                 flags[0] = 1
                 self.epoch_flag_counter = 0
+                self.last_flag = True
             if has_pair0:
                 self.epoch_flag_counter += 1
                 if self.epoch_flag_counter % self.epoch_period == 0:
                     flags = flags | (idx == 0).long()
+                    self.last_flag = True
             out.append(flags)
         return out
 

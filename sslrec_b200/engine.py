@@ -29,6 +29,7 @@ LOG2E = 1.4426950408889634
 # InfoNCE contraction on the wgmma tensor cores (3xTF32, fp32-grade accuracy) when the dim allows; set to False to force
 # the FP32-FMA kernel (tests compare the two)
 USE_TENSOR_CORES = True
+LIVE_ROWS, LIVE_COLS = 1, 2     # SSL_LIVE_ROWS / SSL_LIVE_COLS: which operand of a *_live contraction the device count bounds
 NUM_SM = 132          # H100 SXM; grids of the contraction are sized in resident-CTA slots (kNumSM in csrc/common.cuh)
 
 
@@ -712,7 +713,9 @@ def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_f
     return max(effs, key=lambda t: (round(t[0], 9), -t[1]))[1]
 
 
-def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, deno_eps):
+def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, deno_eps, live=None):
+    """``live``: optional int64 DEVICE scalar; only the first ``*live`` of the ``idx`` rows are anchors (a padded list of
+    capacity idx.numel(), see ``dense_infonce_spec_nodes_mean_dev``).  Shapes and n_split then depend on the capacity only."""
     dev = table.base.device
     d = table.dim
     B, n = idx.numel(), table.n
@@ -723,6 +726,8 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
     p_hat, rinv2 = torch.empty(Bp, d, **f), torch.empty(B, **f)
     comm = table.comm
     full_table = table
+    if live is not None and (comm is not None or not mean):
+        raise RuntimeError('a device-bounded InfoNCE term is a mean on one GPU')
     if comm is not None:                  # contract only this rank's rows of the table; partials are all-reduced
         lo, hi = comm.side_range(table.off, table.n)
         table = table.sub(lo, hi)
@@ -752,10 +757,17 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
                                      _ptr(t_t), rinv_t.data_ptr(), _ptr(t_hi), _ptr(t_lo), _ptr(t_thi), _ptr(t_tlo), npad, s),
               'ssl_rows_normalize(table)')
         with _timed('nce_gemm_fwd', dict(B=B, n=n, dim=d, tc=use_tc)):
-            if use_tc:
+            if use_tc and live is not None:
+                check(lib.ssl_softmax_gemm_tf32x3_live(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), t_thi.data_ptr(),
+                                                       t_tlo.data_ptr(), npad, n, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(),
+                                                       live.data_ptr(), LIVE_ROWS, s), 'ssl_softmax_gemm_tf32x3_live(fwd)')
+            elif use_tc:
                 check(lib.ssl_softmax_gemm_tf32x3(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), t_thi.data_ptr(),
                                                   t_tlo.data_ptr(), npad, n, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(), s),
                       'ssl_softmax_gemm_tf32x3(fwd)')
+            elif live is not None:
+                check(lib.ssl_softmax_gemm_live(a_hat.data_ptr(), B, t_hat.data_ptr(), t_t.data_ptr(), n, d, None, off, n_split,
+                                                rs_part.data_ptr(), o_part.data_ptr(), live.data_ptr(), LIVE_ROWS, s), 'ssl_softmax_gemm_live(fwd)')
             else:
                 check(lib.ssl_softmax_gemm(a_hat.data_ptr(), B, t_hat.data_ptr(), t_t.data_ptr(), n, d, None, off, n_split,
                                            rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm(fwd)')
@@ -766,14 +778,17 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
         check(lib.ssl_nce_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, a_hat.data_ptr(), p_hat.data_ptr(),
                                    tau, deno_eps * math.exp(-1.0 / tau), rowsum.data_ptr(), obar.data_ptr(),
                                    loss_b.data_ptr(), s), 'ssl_nce_finalize')
-        check(lib.ssl_sum(loss_b.data_ptr(), B, (1.0 / B) if mean else 1.0, out.data_ptr(), s), 'ssl_sum')
+        if live is not None:          # (1 / live) sum_{b < live} loss_b: the padding rows' values are never read
+            check(lib.ssl_sum_live(loss_b.data_ptr(), B, live.data_ptr(), 1.0, out.data_ptr(), s), 'ssl_sum_live')
+        else:
+            check(lib.ssl_sum(loss_b.data_ptr(), B, (1.0 / B) if mean else 1.0, out.data_ptr(), s), 'ssl_sum')
     saved = (e1, e2, table, idx, tau, mean, a_hat, a_t, p_hat, rinv1, rinv2, t_hat, rinv_t, rowsum, obar, full_table, comm,
-             (a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo) if use_tc else None)
+             (a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo) if use_tc else None, live)
     return out, saved
 
 
 def _nce_bwd(saved, g):
-    (e1, e2, table, idx, tau, mean, a_hat, a_t, p_hat, rinv1, rinv2, t_hat, rinv_t, rowsum, obar, full_table, comm, tc) = saved
+    (e1, e2, table, idx, tau, mean, a_hat, a_t, p_hat, rinv1, rinv2, t_hat, rinv_t, rowsum, obar, full_table, comm, tc, live) = saved
     dev, d = g.device, table.dim
     B, n = idx.numel(), table.n
     g = g.contiguous()
@@ -787,17 +802,34 @@ def _nce_bwd(saved, g):
             # own rows' dense gradient goes to a compact block that is all-gathered and added to the sink
             local_dt = torch.zeros(comm.side_block(full_table.n), d, **f)
             gt, gt_stride = local_dt.data_ptr(), d
-        if g1 is not None or g2 is not None:
+        if live is not None and (g1 is not None or g2 is not None):        # rows b < live only, mean over live
+            check(lib.ssl_nce_bwd_rows_live(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
+                                            idx.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, g1, e1.stride, g2, e2.stride, s),
+                  'ssl_nce_bwd_rows_live')
+        elif g1 is not None or g2 is not None:
             check(lib.ssl_nce_bwd_rows(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
                                        idx.data_ptr(), B, d, tau, g.data_ptr(), scale, g1, e1.stride, g2, e2.stride, s),
                   'ssl_nce_bwd_rows')
         if gt is not None and n > 0:
             colscale = torch.zeros(ceil_to(B, 64), **f)   # padded tail is read (then masked) by the tile loads
-            check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), scale, colscale.data_ptr(), s), 'ssl_nce_colscale')
+            if live is not None:          # 0 past the live anchors
+                check(lib.ssl_nce_colscale_live(rowsum.data_ptr(), B, live.data_ptr(), g.data_ptr(), 1.0, colscale.data_ptr(), s),
+                      'ssl_nce_colscale_live')
+            else:
+                check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), scale, colscale.data_ptr(), s), 'ssl_nce_colscale')
             n_split = choose_split((n + 127) // 128, ceil_to(B, 64) // 64, slots=NUM_SM if tc else 2 * NUM_SM, prefer_few=bool(tc))
             dt_part = torch.empty(n_split, n, d, **f)
             with _timed('nce_gemm_bwd', dict(B=B, n=n, dim=d, tc=bool(tc))):
-                if tc:
+                if tc and live is not None:
+                    a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo = tc
+                    check(lib.ssl_softmax_gemm_tf32x3_live(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), a_thi.data_ptr(),
+                                                           a_tlo.data_ptr(), a_thi.shape[1], B, d, colscale.data_ptr(), LOG2E / tau, n_split, None,
+                                                           dt_part.data_ptr(), live.data_ptr(), LIVE_COLS, s), 'ssl_softmax_gemm_tf32x3_live(bwd)')
+                elif live is not None:
+                    check(lib.ssl_softmax_gemm_live(t_hat.data_ptr(), n, a_hat.data_ptr(), a_t.data_ptr(), B, d, colscale.data_ptr(),
+                                                    LOG2E / tau, n_split, None, dt_part.data_ptr(), live.data_ptr(), LIVE_COLS, s),
+                          'ssl_softmax_gemm_live(bwd)')
+                elif tc:
                     a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo = tc
                     Bp = a_thi.shape[1]
                     check(lib.ssl_softmax_gemm_tf32x3(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), a_thi.data_ptr(),
@@ -1132,7 +1164,8 @@ class _DenseBprFn(torch.autograd.Function):
 
 class _DenseInfoNceFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, e1, e2, table, idx, idx2, tau, norm_mode, mean, deno_eps, shared_table):
+    def forward(ctx, e1, e2, table, idx, idx2, tau, norm_mode, mean, deno_eps, shared_table, live=None):
+        ctx.n_inputs = 10 if live is None else 11
         r1, s1 = _dense_rows(e1, ctx.needs_input_grad[0])
         if shared_table:                      # e2 rows are rows of the table itself (spec_nodes)
             rt, st_ = _dense_rows(table, ctx.needs_input_grad[2])
@@ -1140,7 +1173,7 @@ class _DenseInfoNceFn(torch.autograd.Function):
         else:
             r2, s2 = _dense_rows(e2, ctx.needs_input_grad[1])
             rt, st_ = _dense_rows(table, ctx.needs_input_grad[2])
-        out, ctx.saved_pack = _nce_fwd(r1, r2, rt, idx, idx2, tau, norm_mode, mean, deno_eps)
+        out, ctx.saved_pack = _nce_fwd(r1, r2, rt, idx, idx2, tau, norm_mode, mean, deno_eps, live)
         ctx.sinks = (s1, s2, st_, shared_table)
         return out
 
@@ -1151,7 +1184,7 @@ class _DenseInfoNceFn(torch.autograd.Function):
         g1 = s1() if s1 is not None else None
         g2 = None if shared else (s2() if s2 is not None else None)
         gt = st_() if st_ is not None else None
-        return g1, g2, gt, None, None, None, None, None, None, None
+        return (g1, g2, gt) + (None,) * (ctx.n_inputs - 3)
 
 
 def dense_bpr_loss_sum(anc, pos, neg):
@@ -1169,6 +1202,30 @@ def dense_infonce_spec_nodes_mean(embeds1, embeds2, nodes, temp):
     """cal_infonce_loss_spec_nodes(embeds1 [N,d], embeds2 [N,d], nodes, temp) -- loss_utils.py:42-51."""
     nodes = _i64(nodes, embeds2.device)
     return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True)
+
+
+def unique_ids(idx: torch.Tensor, n_range: int):
+    """torch.unique(idx, sorted=True) without a host sync or a data-dependent shape: -> (out int64 [n], count int64 device
+    scalar); out[:count] are the distinct ids ascending, out[count:] repeat the largest one.  Every id must be in [0, n_range)."""
+    dev = idx.device
+    idx = _i64(idx, dev).contiguous()
+    words = C.c_int64()
+    check(lib.ssl_unique_ids_scratch(int(n_range), C.byref(words)), 'ssl_unique_ids_scratch')
+    scratch = torch.empty(words.value, dtype=torch.int32, device=dev)
+    out = torch.empty_like(idx)
+    count = torch.empty((), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ssl_unique_ids(idx.data_ptr(), idx.numel(), int(n_range), scratch.data_ptr(), words.value, out.data_ptr(),
+                                 count.data_ptr(), _stream(idx)), 'ssl_unique_ids')
+    return out, count
+
+
+def dense_infonce_spec_nodes_mean_dev(embeds1, embeds2, ids, temp):
+    """The graph-safe form of ``dense_infonce_spec_nodes_mean(embeds1, embeds2, torch.unique(ids), temp)``: the unique ids are
+    found on the device (``unique_ids``), the term runs over the padded list at capacity ids.numel() and every piece is bounded
+    by the device count -- no host read, no data-dependent shape, so a CUDA graph can capture it."""
+    nodes, count = unique_ids(ids, embeds2.shape[0])
+    return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, count)
 
 
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------

@@ -70,14 +70,20 @@ class HCCF(BaseModel):
 
     def _contrast(self, gcn_out, hyper_out, ancs, poss):
         """sum over layers and sides of the spec-node InfoNCE between the DETACHED SpMM output and the hyper output on the
-        batch's unique users / items (hccf.py:76-81)."""
+        batch's unique users / items (hccf.py:76-81).  Driven by a graphed.GraphedStep (``_graph_mode``), the de-duplication
+        runs on the device and the term is bounded by the device count: no host sync, no data-dependent shape."""
         nu = self.user_num
-        picks = ((slice(0, nu), torch.unique(ancs)), (slice(nu, None), torch.unique(poss)))
+        if getattr(self, '_graph_mode', False):
+            picks = ((slice(0, nu), ancs), (slice(nu, None), poss))
+            term = E.dense_infonce_spec_nodes_mean_dev
+        else:
+            picks = ((slice(0, nu), torch.unique(ancs)), (slice(nu, None), torch.unique(poss)))
+            term = cal_infonce_loss_spec_nodes
         total = 0
         for g, h in zip(gcn_out, hyper_out):
             g = g.detach()
             for rows, nodes in picks:
-                total = total + cal_infonce_loss_spec_nodes(g[rows], h[rows], nodes, self.temperature)
+                total = total + term(g[rows], h[rows], nodes, self.temperature)
         return total
 
     def cal_loss(self, batch_data):

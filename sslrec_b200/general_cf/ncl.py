@@ -27,6 +27,21 @@ class NCL(LightGCN):
         self.user_centroids, self.user2cluster, _ = self.kmeans(self.user_embeds.detach())     # ncl.py:26-28
         self.item_centroids, self.item2cluster, _ = self.kmeans(self.item_embeds.detach())
 
+    def graph_pre_step(self, recluster: bool) -> None:
+        """Run by graphed.GraphedStep before every step, outside the captured region: the re-clustering that the eager
+        ``cal_loss`` does when the batch's k-means flag is set (and on the first step).  The results are copied IN PLACE into
+        the buffers of the first clustering, so a captured step keeps reading the current centroids and assignments."""
+        if hasattr(self, 'user2cluster') and not recluster:
+            return
+        first = not hasattr(self, 'user2cluster')
+        old = None if first else (self.user_centroids, self.user2cluster, self.item_centroids, self.item2cluster)
+        self._cluster()
+        if old is not None:
+            new = (self.user_centroids, self.user2cluster, self.item_centroids, self.item2cluster)
+            for dst, src in zip(old, new):
+                dst.copy_(src)
+            self.user_centroids, self.user2cluster, self.item_centroids, self.item2cluster = old
+
     def _run(self):
         ctx_layer = self.high_order * 2
         iteration = max(self.layer_num, ctx_layer)                                              # ncl.py:36
@@ -44,7 +59,8 @@ class NCL(LightGCN):
     def cal_loss(self, batch_data):
         self.is_training = True
         ancs, poss, negs, kmeans_flags = batch_data
-        if not hasattr(self, 'user2cluster') or bool(torch.sum(kmeans_flags) != 0):             # ncl.py:73-74
+        # ncl.py:73-74; driven by a graphed.GraphedStep the flag is decided on the host and graph_pre_step clusters
+        if not getattr(self, '_graph_mode', False) and (not hasattr(self, 'user2cluster') or bool(torch.sum(kmeans_flags) != 0)):
             self._cluster()
         embeds, st = self.forward(self.adj)
         ctx = self.high_order * 2

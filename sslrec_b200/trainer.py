@@ -73,9 +73,10 @@ class Trainer(object):
         if use_graph and self.grad_sync is not None:
             raise RuntimeError('train.cuda_graph captures a single-GPU step (no gradient exchange inside)')
         for _, tem in enumerate(train_dataloader):
+            recluster = _recluster_flag(train_dataloader, tem) if use_graph else False
             batch_data = list(map(lambda x: x.long().to(configs['device'], non_blocking=True), tem))
             if use_graph:
-                loss, loss_dict = self._graph_step(model, batch_data)
+                loss, loss_dict = self._graph_step(model, batch_data, recluster)
             else:
                 self.optimizer.zero_grad()
                 loss, loss_dict = model.cal_loss(batch_data)
@@ -97,21 +98,22 @@ class Trainer(object):
             self.logger.log_loss(epoch_idx, loss_log_dict, save_to_log=configs['train'].get('log_loss', True))
         return ep_loss, loss_log_dict
 
-    def _graph_step(self, model, batch_data):
+    def _graph_step(self, model, batch_data, recluster=False):
         """The step through graphed.GraphedStep: the first full-size batch is stepped eagerly (that is the capture's warm-up -- every
         batch is trained on exactly once, like the eager loop) and captured; later full-size batches replay the graph; a batch of
-        another size (the epoch's last) runs eagerly with the same device-resident seeds."""
+        another size (the epoch's last) runs eagerly with the same device-resident seeds.  ``recluster``: the batch carries NCL's
+        k-means flag (decided on the host), so the model re-clusters before the step, outside the graph."""
         from .graphed import GraphedStep
         g = self._graphed
         if g is not None and g.model is not model:
             g.close()
             g = self._graphed = None
         if g is None:
-            g = self._graphed = GraphedStep(model, self.optimizer, batch_data, warmup=1)
+            g = self._graphed = GraphedStep(model, self.optimizer, batch_data, warmup=1, recluster=recluster)
             return g.warm_result
         if all(a.shape == b.shape for a, b in zip(batch_data, g.static_batch)):
-            return g(batch_data)
-        return g.eager(batch_data)
+            return g(batch_data, recluster=recluster)
+        return g.eager(batch_data, recluster=recluster)
 
     def train(self, model):
         """trainer.py:86-137: plain run (evaluate every ``test_step`` epochs, then test + save) or, when the YAML
@@ -241,6 +243,18 @@ class Trainer(object):
         if self.logger is not None:
             self.logger.log_eval(result, ks, data_type=data_type or 'Validation set', epoch_idx=epoch_idx)
         return result
+
+
+def _recluster_flag(loader, tem) -> bool:
+    """Whether a training batch carries NCL's k-means flag (its 4th tensor, datasets_general_cf.py:28-44), without a device read:
+    host loaders hold the flags in host memory; a DeviceTrnData knows on the host which batch got a set flag (its loader reads
+    where pair 0 landed once per epoch)."""
+    if len(tem) < 4:
+        return False
+    flags = tem[3]
+    if not flags.is_cuda:
+        return bool(flags.any())
+    return bool(getattr(loader.dataset, 'last_flag', False))
 
 
 def _eval_batches(loader):
