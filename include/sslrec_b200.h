@@ -356,6 +356,18 @@ SSL_API int ssl_predict_mask(const float *users_tab, int64_t u_stride, const flo
 SSL_API int ssl_spmm_exact(const int32_t *rowptr, const int32_t *colidx, const float *vals, int64_t n_rows, const float *x, int64_t x_stride,
                    int32_t dim, float *y, int64_t y_stride, void *stream);
 SSL_API int ssl_topk(const float *preds, int64_t n_b, int64_t n_item, int32_t k, int64_t *out_idx, float *out_val, void *stream);
+/* ssl_predict_topk: ssl_predict_mask followed by ssl_topk in one call, without the [n_b, n_item] score matrix: out_idx int64 [n_b, k]
+ *   and, when out_val is not NULL, out_val fp32 [n_b, k] are bit-identical to that pair on the same inputs.  Each score is formed by the
+ *   same FMA chain and masked by the same formula, and rows are ranked by the same total key (value descending, then item ascending),
+ *   so the result does not depend on scheduling.  Arguments as ssl_predict_mask; the training CSR rows must be sorted ascending.
+ *   1 <= k <= min(256, n_item), n_b <= 65535.  workspace: ws_bytes >= what ssl_predict_topk_workspace reports for (n_b, n_item, k),
+ *   16-byte aligned, owned by the caller and not required to be initialised (it is O(n_b * (2k + 128)) bytes per item chunk, at most
+ *   264 / ceil(n_b / 128) chunks).  Bad arguments return SSL_E_ARG before anything is written. */
+SSL_API int ssl_predict_topk_workspace(int64_t n_b, int64_t n_item, int32_t k, int64_t *bytes);
+SSL_API int ssl_predict_topk(const float *users_tab, int64_t u_stride, const float *items_tab, int64_t i_stride, const int64_t *users,
+                     int64_t n_b, int64_t n_item, int32_t dim, const int64_t *mask_dense, const int32_t *trn_rowptr,
+                     const int32_t *trn_cols, int32_t k, void *workspace, int64_t ws_bytes, int64_t *out_idx, float *out_val,
+                     void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * SURVEY 8(f) row 4  DirectAU's losses (loss_utils.py:75-86) on unit rows x^ = F.normalize(x)

@@ -94,6 +94,8 @@ def _load():
         'ssl_hyper_dropout_dev': (C.c_int, [vp, vp, i64, i32, f32, i32, vp, vp, C.c_uint32, i32, vp]),
         'ssl_predict_mask': (C.c_int, [vp, i64, vp, i64, vp, i64, i64, i32, vp, vp, vp, vp, vp]),
         'ssl_topk': (C.c_int, [vp, i64, i64, i32, vp, vp, vp]),
+        'ssl_predict_topk_workspace': (C.c_int, [i64, i64, i32, c_i64p]),
+        'ssl_predict_topk': (C.c_int, [vp, i64, vp, i64, vp, i64, i64, i32, vp, vp, vp, i32, vp, i64, vp, vp, vp]),
         'ssl_spmm_exact': (C.c_int, [vp, vp, vp, i64, vp, i64, i32, vp, i64, vp]),
         'ssl_align_fwd': (C.c_int, [vp, vp, i64, i32, vp, vp]),
         'ssl_uniform_finalize': (C.c_int, [vp, vp, i32, i64, i32, vp, vp, f32, vp, vp, vp]),

@@ -2,6 +2,8 @@
 ``_mask_predict`` formula), plus the flat embedding table the kernels read without a concat."""
 from __future__ import annotations
 
+import ctypes as C
+
 import torch
 from torch import nn
 
@@ -136,18 +138,9 @@ class BaseModel(nn.Module):
         """E_u[users] E_i^T with the training positives masked to -1e8 (lightgcn.py:61-65, base_model.py:35-36) in
         one kernel; no [Bt, I] temporaries besides the result.  ``train_mask``: the reference's dense [Bt, I] 0/1
         tensor, or None = no masking, or the string 'train' = mask the user's training items from the device CSR."""
-        # [users] alone (a lean AllRankTstData batch driven by the reference's Metric.eval, metrics.py:94-101) = mask from the device CSR
-        pck_users, train_mask = (batch_data[0], 'train') if len(batch_data) == 1 else batch_data
-        pck_users = pck_users.long().contiguous()
+        pck_users, mask, rowptr, cols = self._eval_batch(batch_data, user_embeds.device)
         n_b = pck_users.shape[0]
         preds = torch.empty(n_b, self.item_num, device=user_embeds.device, dtype=torch.float32)
-        mask, rowptr, cols = None, None, None
-        if isinstance(train_mask, str):
-            if train_mask != 'train' or getattr(self, '_trn_mat', None) is None:
-                raise ValueError("train_mask must be a tensor, None or 'train' (needs data_handler.trn_mat)")
-            rowptr, cols = self._train_csr(preds.device)
-        elif train_mask is not None:
-            mask = train_mask.long().contiguous()
         with torch.cuda.device(preds.device):
             check(lib.ssl_predict_mask(user_embeds.data_ptr(), user_embeds.stride(0), item_embeds.data_ptr(), item_embeds.stride(0),
                                        pck_users.data_ptr(), n_b, self.item_num, self.embedding_size,
@@ -155,3 +148,36 @@ class BaseModel(nn.Module):
                                        None if cols is None else cols.data_ptr(), preds.data_ptr(),
                                        torch.cuda.current_stream(preds.device).cuda_stream), 'ssl_predict_mask')
         return preds
+
+    def _eval_batch(self, batch_data, device):
+        """An evaluation batch -> (users int64, dense mask | None, CSR rowptr | None, CSR cols | None)."""
+        # [users] alone (a lean AllRankTstData batch driven by the reference's Metric.eval, metrics.py:94-101) = mask from the device CSR
+        pck_users, train_mask = (batch_data[0], 'train') if len(batch_data) == 1 else batch_data
+        pck_users = pck_users.long().contiguous()
+        mask, rowptr, cols = None, None, None
+        if isinstance(train_mask, str):
+            if train_mask != 'train' or getattr(self, '_trn_mat', None) is None:
+                raise ValueError("train_mask must be a tensor, None or 'train' (needs data_handler.trn_mat)")
+            rowptr, cols = self._train_csr(device)
+        elif train_mask is not None:
+            mask = train_mask.long().contiguous()
+        return pck_users, mask, rowptr, cols
+
+    def _predict_topk(self, user_embeds, item_embeds, batch_data, k, return_values=False):
+        """``trainer.topk(self._predict(user_embeds, item_embeds, batch_data), k, return_values)`` -- the same ids and values bit for
+        bit -- ranked on the device without the [Bt, I] score matrix: only the call's workspace and the [Bt, k] outputs are allocated."""
+        dev = user_embeds.device
+        pck_users, mask, rowptr, cols = self._eval_batch(batch_data, dev)
+        n_b = pck_users.shape[0]
+        ws_bytes = C.c_int64(0)
+        check(lib.ssl_predict_topk_workspace(n_b, self.item_num, k, C.byref(ws_bytes)), 'ssl_predict_topk_workspace')
+        ws = torch.empty(ws_bytes.value, device=dev, dtype=torch.uint8)
+        idx = torch.empty(n_b, k, device=dev, dtype=torch.int64)
+        val = torch.empty(n_b, k, device=dev, dtype=torch.float32) if return_values else None
+        with torch.cuda.device(dev):
+            check(lib.ssl_predict_topk(user_embeds.data_ptr(), user_embeds.stride(0), item_embeds.data_ptr(), item_embeds.stride(0),
+                                       pck_users.data_ptr(), n_b, self.item_num, self.embedding_size,
+                                       None if mask is None else mask.data_ptr(), None if rowptr is None else rowptr.data_ptr(),
+                                       None if cols is None else cols.data_ptr(), k, ws.data_ptr(), ws_bytes.value, idx.data_ptr(),
+                                       None if val is None else val.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), 'ssl_predict_topk')
+        return (idx, val) if return_values else idx

@@ -47,7 +47,14 @@ class DirectAU(BaseModel):
         losses = {'align_loss': align_loss, 'uniform_loss': uniform_loss}
         return loss, losses
 
-    def full_predict(self, batch_data):
+    def _eval_tables(self):
         user_embeds, item_embeds = self.forward(self.adj)
         self.is_training = False
-        return self._predict(user_embeds, item_embeds, batch_data)
+        return user_embeds, item_embeds
+
+    def full_predict(self, batch_data):
+        return self._predict(*self._eval_tables(), batch_data)
+
+    def predict_topk(self, batch_data, k, return_values=False):
+        """``topk(full_predict(batch_data), k, return_values)`` without the [Bt, I] score matrix (same ids and values)."""
+        return self._predict_topk(*self._eval_tables(), batch_data, k, return_values)

@@ -96,9 +96,16 @@ class HCCF(BaseModel):
                  'cl_loss': self._contrast(gcn_out, hyper_out, ancs, poss) * self.cl_weight}
         return terms['bpr_loss'] + terms['reg_loss'] + terms['cl_loss'], terms
 
-    def full_predict(self, batch_data):
+    def _eval_tables(self):
         embeds, _, _ = self.forward(self.adj, 1.0)
-        return self._predict(embeds[:self.user_num], embeds[self.user_num:], batch_data)
+        return embeds[:self.user_num], embeds[self.user_num:]
+
+    def full_predict(self, batch_data):
+        return self._predict(*self._eval_tables(), batch_data)
+
+    def predict_topk(self, batch_data, k, return_values=False):
+        """``topk(full_predict(batch_data), k, return_values)`` without the [Bt, I] score matrix (same ids and values)."""
+        return self._predict_topk(*self._eval_tables(), batch_data, k, return_values)
 
 
 class HGNNLayer(nn.Module):

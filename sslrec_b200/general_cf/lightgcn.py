@@ -90,7 +90,15 @@ class LightGCN(BaseModel):
             return self._exact_forward()
         return forward()
 
-    def full_predict(self, batch_data):
+    def _eval_tables(self):
+        """The (user, item) tables evaluation scores with, with full_predict's side effects (``is_training``, the cache)."""
         user_embeds, item_embeds = self._eval_embeds(lambda: self.forward(self.adj, 1.0))
         self.is_training = False
-        return self._predict(user_embeds, item_embeds, batch_data)
+        return user_embeds, item_embeds
+
+    def full_predict(self, batch_data):
+        return self._predict(*self._eval_tables(), batch_data)
+
+    def predict_topk(self, batch_data, k, return_values=False):
+        """``topk(full_predict(batch_data), k, return_values)`` without the [Bt, I] score matrix (same ids and values)."""
+        return self._predict_topk(*self._eval_tables(), batch_data, k, return_values)

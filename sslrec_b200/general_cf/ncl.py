@@ -80,11 +80,11 @@ class NCL(LightGCN):
         losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'struct_loss': struct_loss, 'proto_loss': proto_loss}
         return loss, losses
 
-    def full_predict(self, batch_data):
+    def _eval_tables(self):
         if configs.get('test', {}).get('exact_order', False):        # the evaluation embeddings are the sum of the first layer_num + 1 outputs (ncl.py:40-41)
             user_embeds, item_embeds = self._exact_forward()
         else:
             embeds, _ = self.forward(self.adj)
             user_embeds, item_embeds = embeds[:self.user_num], embeds[self.user_num:]
         self.is_training = False
-        return self._predict(user_embeds, item_embeds, batch_data)
+        return user_embeds, item_embeds

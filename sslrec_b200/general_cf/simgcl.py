@@ -44,7 +44,7 @@ class SimGCL(LightGCN):
         losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
         return loss, losses
 
-    def full_predict(self, batch_data):
+    def _eval_tables(self):
         user_embeds, item_embeds = self._eval_embeds(lambda: self.forward(self.adj, False))
         self.is_training = False
-        return self._predict(user_embeds, item_embeds, batch_data)
+        return user_embeds, item_embeds

@@ -15,6 +15,11 @@ from ._lib import check, lib
 from .config import configs
 from .optim import FusedAdam
 
+# Trainer.evaluate ranks with model.predict_topk (no [Bt, I] score matrix) from this many items on, below it with full_predict + topk; both
+# give the same ids.  On an H100 80GB HBM3 (400 W and 700 W, profiles/r06_predict_topk.md) the fused call runs at 0.55-0.91x the pair's
+# speed at 19 747-83 761 items and 1.3-1.5x it at 1 000 000 items (256- and 1024-user batches); the crossover in between is not measured.
+FUSED_TOPK_MIN_ITEMS = 1_000_000
+
 
 def init_seed():
     """trainer/trainer.py:26-36."""
@@ -201,7 +206,8 @@ class Trainer(object):
 
     @torch.no_grad()
     def evaluate(self, model, epoch_idx=None, loader=None, data_type=None):
-        """All-rank evaluation: full_predict -> top-max(k) on device -> recall / ndcg / precision / mrr on host
+        """All-rank evaluation: full_predict -> top-max(k) on device (one fused predict_topk call when the model has it and the catalogue
+        has at least FUSED_TOPK_MIN_ITEMS items) -> recall / ndcg / precision / mrr on host
         (metrics.py:11-45, :82-127).  Validation split when the handler has one, else the test split
         (trainer.py:139-150)."""
         model.eval()
@@ -229,9 +235,12 @@ class Trainer(object):
             batch_data = list(map(lambda x: x.long().to(configs['device']), tem))
             if len(batch_data) == 1:
                 batch_data.append('train')                   # dataset built with dense_mask=False: mask from the device CSR
-            preds = model.full_predict(batch_data)
-            seen += preds.shape[0]
-            top = topk(preds, max(ks)).cpu().numpy()
+            if hasattr(model, 'predict_topk') and getattr(model, 'item_num', 0) >= FUSED_TOPK_MIN_ITEMS:     # the same ids either way
+                top = model.predict_topk(batch_data, max(ks))
+            else:
+                top = topk(model.full_predict(batch_data), max(ks))
+            seen += top.shape[0]
+            top = top.cpu().numpy()
             rows = batch_metric_rows(top, users, ptr, flat, ks, metrics)
             for m in metrics:
                 per_user[m].append(rows[m])
