@@ -233,6 +233,21 @@ SSL_API int ssl_softmax_gemm_tf32x3(const float *R_hi, const float *R_lo, int64_
                             const float *CT_hi, const float *CT_lo, int64_t ct_pitch, int64_t n_c, int32_t dim,
                             const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                             void *stream);
+/* The same contraction at the FP16 tensor-core rate with 3xFP16 error compensation (fp32-grade accuracy, the grade of
+ * ssl_softmax_gemm_tf32x3).  Operands are the fp16 bit patterns written by ssl_rows_normalize_f16x3: for each operand
+ * x = hi + 2^-12 lo, hi = fp16(x) (0 below 2^-14), lo = fp16((x - hi) 2^12), row-major [n, dim].  No transposed copy.
+ * The split's bounds (derived in csrc/f16x3.cuh) need rows of norm <= 1 scaled by |alpha| <= 16 and
+ * R_r . C_c <= offset, with 0 <= offset <= 16 (tau >= 0.0902 in the InfoNCE roles); an offset outside [0, 16] is
+ * rejected.  colscale may take any magnitude: the kernel rescales it by a power of two found on the device.
+ * dim must be 32 or 64.  Outputs and semantics are those of ssl_softmax_gemm. */
+SSL_API int ssl_softmax_gemm_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo,
+                           int64_t n_c, int32_t dim, const float *colscale, float offset, int32_t n_split, float *rowsum_part,
+                           float *o_part, void *stream);
+/* ssl_rows_normalize (norm_mode 0, 1 or 2, |alpha| <= 16, dim 32 or 64) writing out [n, dim] and rinv [n] as it does,
+ * plus the operands of ssl_softmax_gemm_f16x3: out_hi / out_lo, fp16 [ceil64(n), dim] each, rows n .. ceil64(n) zero
+ * (out must hold ceil64(n) rows as well). */
+SSL_API int ssl_rows_normalize_f16x3(const float *x, int64_t stride, const int64_t *idx, int64_t n, int32_t dim, int32_t norm_mode,
+                             float alpha, float *out, float *rinv, uint16_t *out_hi, uint16_t *out_lo, void *stream);
 /* forward epilogue of one term: reduces the split partials and produces, per anchor b,
  *   rowsum[b] (+ deno_eps), obar[b,:] = o[b,:]/rowsum[b] and
  *   loss_b[b] = -(a^_b . p^_b)/tau + 1/tau + ln(rowsum[b])          */
@@ -262,7 +277,7 @@ SSL_API int ssl_nce_colscale(const float *rowsum, int64_t batch, const float *gs
  * ssl_unique_ids).  n_live points to an int64 on the device, clamped to [0, capacity]; the host
  * passes the capacity, so buffer shapes, tensor maps and n_split depend on host-known sizes only.
  *
- * ssl_softmax_gemm_live / ssl_softmax_gemm_tf32x3_live: the contractions above, with
+ * ssl_softmax_gemm_live / ssl_softmax_gemm_tf32x3_live / ssl_softmax_gemm_f16x3_live: the contractions above, with
  *   live_role SSL_LIVE_ROWS: only rows r < *n_live of R are live (the forward, R = anchors).  Their
  *     outputs equal those of the plain call at n_r = *n_live bit for bit; rows >= *n_live of
  *     o_part / rowsum_part are not written (the row pitch stays n_r).  Units whose R tile starts
@@ -285,6 +300,10 @@ SSL_API int ssl_softmax_gemm_tf32x3_live(const float *R_hi, const float *R_lo, i
                                  const float *CT_hi, const float *CT_lo, int64_t ct_pitch, int64_t n_c, int32_t dim,
                                  const float *colscale, float offset, int32_t n_split, float *rowsum_part, float *o_part,
                                  const int64_t *n_live, int32_t live_role, void *stream);
+SSL_API int ssl_softmax_gemm_f16x3_live(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi,
+                                const uint16_t *C_lo, int64_t n_c, int32_t dim, const float *colscale, float offset,
+                                int32_t n_split, float *rowsum_part, float *o_part, const int64_t *n_live, int32_t live_role,
+                                void *stream);
 SSL_API int ssl_sum_live(const float *x, int64_t n, const int64_t *n_live, float alpha, float *out, void *stream);
 SSL_API int ssl_nce_bwd_rows_live(const float *a_hat, const float *p_hat, const float *obar, const float *rinv1, const float *rinv2,
                           const int64_t *idx, int64_t batch, const int64_t *n_live, int32_t dim, float tau, const float *gscale,

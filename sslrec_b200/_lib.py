@@ -68,6 +68,9 @@ def _load():
         'ssl_bpr_bwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, vp, vp, f32, vp, i64, vp, i64, vp]),
         'ssl_rows_normalize': (C.c_int, [vp, i64, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp, vp, vp, i64, vp]),
         'ssl_softmax_gemm_tf32x3': (C.c_int, [vp, vp, i64, vp, vp, vp, vp, i64, i64, i32, vp, f32, i32, vp, vp, vp]),
+        'ssl_rows_normalize_f16x3': (C.c_int, [vp, i64, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp]),
+        'ssl_softmax_gemm_f16x3': (C.c_int, [vp, vp, i64, vp, vp, i64, i32, vp, f32, i32, vp, vp, vp]),
+        'ssl_softmax_gemm_f16x3_live': (C.c_int, [vp, vp, i64, vp, vp, i64, i32, vp, f32, i32, vp, vp, vp, i32, vp]),
         'ssl_softmax_gemm': (C.c_int, [vp, i64, vp, vp, i64, i32, vp, f32, i32, vp, vp, vp]),
         'ssl_nce_finalize': (C.c_int, [vp, vp, i32, i64, i32, vp, vp, f32, f32, vp, vp, vp, vp]),
         'ssl_lse_finalize': (C.c_int, [vp, vp, i32, i64, i32, f32, vp, vp, vp, vp]),

@@ -4,6 +4,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
+#include "f16x3.cuh"
 #include "predict_tile.cuh"
 
 namespace {
@@ -137,6 +138,48 @@ __global__ void __launch_bounds__(256) rows_normalize_kernel(const float *__rest
             ssl::tf32_split(tile[c * pitch + k], hi, lo);
             out_thi[(size_t)k * t_pitch + row0 + q] = hi;
             out_tlo[(size_t)k * t_pitch + row0 + q] = lo;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// rows_normalize_f16x3: the operands of ssl_softmax_gemm_f16x3.  rows_normalize's row-major copy and 1/norm (the same
+// arithmetic, so ``out`` and ``rinv`` are bit-identical to it), plus the f16x3 split of the output (f16x3.cuh) as
+// row-major fp16 hi / lo [ceil64(n), dim].  No transposed copy: the contraction reads the row-major tile both ways.
+// One 64-row tile per block, one warp per row; rows n .. ceil64(n) are written as zeros.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) rows_normalize_f16x3_kernel(const float *__restrict__ x, int64_t stride, const int64_t *__restrict__ idx,
+                                                                 int64_t n, int dim, int mode, float alpha, float *__restrict__ out,
+                                                                 float *__restrict__ rinv, __half *__restrict__ out_hi,
+                                                                 __half *__restrict__ out_lo) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t row0 = (int64_t)blockIdx.x * 64;
+    for (int lr = warp; lr < 64; lr += 8) {
+        const int64_t row = row0 + lr;
+        float v[kMaxPerLane];
+        float ri = 0.f;
+        if (row < n) {
+            const int64_t src = idx ? idx[row] : row;
+            load_row(x + src * stride, dim, lane, v);
+            if (mode == 1) {
+#pragma unroll
+                for (int i = 0; i < kMaxPerLane; ++i) if (lane + 32 * i < dim) v[i] += 1e-8f;    // F.normalize(x + 1e-8)
+            }
+            const float ss = dot_rows(v, v);
+            ri = (mode == 0) ? (1.f / sqrtf(1e-8f + ss)) : (1.f / fmaxf(sqrtf(ss), 1e-12f));
+            if (lane == 0 && rinv) rinv[row] = ri;
+        } else {
+#pragma unroll
+            for (int i = 0; i < kMaxPerLane; ++i) v[i] = 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < kMaxPerLane; ++i) {
+            const int k = lane + 32 * i;
+            if (k < dim) {
+                const float y = v[i] * ri * alpha;
+                out[row * dim + k] = y;
+                ssl::f16x3_split1(y, out_hi[row * dim + k], out_lo[row * dim + k]);
+            }
         }
     }
 }
@@ -489,6 +532,21 @@ extern "C" int ssl_rows_normalize(const float *x, int64_t stride, const int64_t 
     const size_t smem = sizeof(float) * 64 * (dim + 1);
     rows_normalize_kernel<<<(unsigned)((n + 63) / 64), 256, smem, STREAM>>>(x, stride, idx, n, dim, norm_mode, alpha, out, out_t, rinv, out_hi, out_lo, out_thi, out_tlo, t_pitch);
     SSL_LAUNCH_CHECK("rows_normalize_kernel");
+    return SSL_OK;
+}
+
+extern "C" int ssl_rows_normalize_f16x3(const float *x, int64_t stride, const int64_t *idx, int64_t n, int32_t dim, int32_t norm_mode,
+                                        float alpha, float *out, float *rinv, uint16_t *out_hi, uint16_t *out_lo, void *stream) {
+    SSL_CHECK_ARG(x && out && out_hi && out_lo, "ssl_rows_normalize_f16x3: null argument");
+    SSL_CHECK_ARG(dim == 32 || dim == 64, "ssl_rows_normalize_f16x3: dim %d not supported (32 or 64)", dim);
+    SSL_CHECK_ARG(norm_mode >= 0 && norm_mode <= 2, "ssl_rows_normalize_f16x3: norm_mode %d (0, 1 or 2: unit rows only)", norm_mode);
+    SSL_CHECK_ARG(fabsf(alpha) <= ssl::kF16MaxAlpha, "ssl_rows_normalize_f16x3: |alpha| = %g exceeds %g", (double)fabsf(alpha),
+                  (double)ssl::kF16MaxAlpha);
+    if (n == 0) return SSL_OK;
+    rows_normalize_f16x3_kernel<<<(unsigned)((n + 63) / 64), 256, 0, STREAM>>>(x, stride, idx, n, dim, norm_mode, alpha, out, rinv,
+                                                                               reinterpret_cast<__half *>(out_hi),
+                                                                               reinterpret_cast<__half *>(out_lo));
+    SSL_LAUNCH_CHECK("rows_normalize_f16x3_kernel");
     return SSL_OK;
 }
 

@@ -26,11 +26,19 @@ from ._lib import PropArgs, check, lib
 from .graph import GraphPlan
 
 LOG2E = 1.4426950408889634
-# InfoNCE contraction on the wgmma tensor cores (3xTF32, fp32-grade accuracy) when the dim allows; set to False to force
-# the FP32-FMA kernel (tests compare the two)
+# InfoNCE contraction on the wgmma tensor cores (3xFP16 or 3xTF32, fp32-grade accuracy) when the dim allows; set to False
+# to force the FP32-FMA kernel (tests compare the two)
 USE_TENSOR_CORES = True
+# ssl_softmax_gemm_f16x3 accepts unit rows scaled by |alpha| <= 16 and offsets in [0, 16] (csrc/f16x3.cuh): every InfoNCE
+# temperature >= 0.0902 and the uniformity term.  Raw rows (LightGCL) and larger offsets keep the 3xTF32 kernel.
+F16X3_MAX_OFFSET = 16.0
 LIVE_ROWS, LIVE_COLS = 1, 2     # SSL_LIVE_ROWS / SSL_LIVE_COLS: which operand of a *_live contraction the device count bounds
 NUM_SM = 132          # H100 SXM; grids of the contraction are sized in resident-CTA slots (kNumSM in csrc/common.cuh)
+
+
+def f16x3_applies(offset: float) -> bool:
+    """True when the 3xFP16 contraction's operand bound holds for a term with this offset (rows normalised by the engine)."""
+    return 0.0 <= offset <= F16X3_MAX_OFFSET
 
 
 def _stream(t: torch.Tensor) -> int:
@@ -694,8 +702,9 @@ def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_f
 
     ``prefer_few`` (the persistent tensor-core kernel, one CTA per SM looping over n_rtiles * n_split units): minimise
     rounds(s) * (tiles_per_unit(s) + c)  with c = 5 tile-times of per-unit overhead (R fragment load, pipeline restart,
-    O write-out), fitted to an n_split sweep of that kernel at the amazon forward shape on an H100 (profiles/r04_nce_tc.md);
-    fewer, longer units than the pure wave-efficiency rule picks.  The split only changes how the work is cut, never the
+    O write-out), fitted to an n_split sweep of that kernel at the amazon forward shape on an H100 (profiles/r04_nce_tc.md;
+    the sweep of the 3xFP16 kernel in profiles/r07_nce_f16x3.md fits the same c); fewer, longer units than the pure
+    wave-efficiency rule picks.  The split only changes how the work is cut, never the
     result beyond summation order.
     Otherwise: the split with the best wave efficiency (FFMA kernel)."""
     max_split = max(1, min(n_ctiles // 4 if n_ctiles >= 4 else 1, 64))
@@ -733,31 +742,51 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
         table = table.sub(lo, hi)
         n = table.n
         npad = max(64, ceil_to(n, 64))
-    use_tc = USE_TENSOR_CORES and d in (32, 64)     # tensor-core 3xTF32 contraction; other dims run the FFMA kernel
+    off = LOG2E / tau
+    use_tc = USE_TENSOR_CORES and d in (32, 64)     # tensor-core contraction; other dims run the FFMA kernel
+    f16 = use_tc and f16x3_applies(off)              # 3xFP16 where its operand bound holds, else 3xTF32
     t_hat, rinv_t = torch.empty(npad, d, **f), torch.empty(max(n, 1), **f)
-    if use_tc:
-        a_t = t_t = None
+    a_hi = a_lo = t_hi = t_lo = a_thi = a_tlo = t_thi = t_tlo = t_t = None
+    if f16:
+        a_t = None
+        h = dict(device=dev, dtype=torch.float16)
+        a_hi, a_lo, t_hi, t_lo = torch.empty(Bp, d, **h), torch.empty(Bp, d, **h), torch.empty(npad, d, **h), torch.empty(npad, d, **h)
+    elif use_tc:
+        a_t = None
         a_hi, a_lo, a_thi, a_tlo = torch.empty(Bp, d, **f), torch.empty(Bp, d, **f), torch.empty(d, Bp, **f), torch.empty(d, Bp, **f)
         t_hi, t_lo, t_thi, t_tlo = torch.empty(npad, d, **f), torch.empty(npad, d, **f), torch.empty(d, npad, **f), torch.empty(d, npad, **f)
     else:
         t_t = torch.empty(npad // 64, d, 64, **f)
-        a_hi = a_lo = t_hi = t_lo = a_thi = a_tlo = t_thi = t_tlo = None
     n_split = choose_split((B + 127) // 128, npad // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
     rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
     rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
-    off = LOG2E / tau
     with torch.cuda.device(dev):
         s = _stream(table.base)
-        check(lib.ssl_rows_normalize(e1.ptr, e1.stride, idx.data_ptr(), B, d, norm_mode, off, a_hat.data_ptr(),
-                                     _ptr(a_t), rinv1.data_ptr(), _ptr(a_hi), _ptr(a_lo), _ptr(a_thi), _ptr(a_tlo), Bp, s),
-              'ssl_rows_normalize(e1)')
+        if f16:
+            check(lib.ssl_rows_normalize_f16x3(e1.ptr, e1.stride, idx.data_ptr(), B, d, norm_mode, off, a_hat.data_ptr(),
+                                               rinv1.data_ptr(), a_hi.data_ptr(), a_lo.data_ptr(), s), 'ssl_rows_normalize_f16x3(e1)')
+        else:
+            check(lib.ssl_rows_normalize(e1.ptr, e1.stride, idx.data_ptr(), B, d, norm_mode, off, a_hat.data_ptr(),
+                                         _ptr(a_t), rinv1.data_ptr(), _ptr(a_hi), _ptr(a_lo), _ptr(a_thi), _ptr(a_tlo), Bp, s),
+                  'ssl_rows_normalize(e1)')
         check(lib.ssl_rows_normalize(e2.ptr, e2.stride, idx2.data_ptr(), B, d, norm_mode, 1.0, p_hat.data_ptr(), None,
                                      rinv2.data_ptr(), None, None, None, None, 0, s), 'ssl_rows_normalize(e2)')
-        check(lib.ssl_rows_normalize(table.ptr, table.stride, None, n, d, norm_mode, 1.0, t_hat.data_ptr(),
-                                     _ptr(t_t), rinv_t.data_ptr(), _ptr(t_hi), _ptr(t_lo), _ptr(t_thi), _ptr(t_tlo), npad, s),
-              'ssl_rows_normalize(table)')
+        if f16:
+            check(lib.ssl_rows_normalize_f16x3(table.ptr, table.stride, None, n, d, norm_mode, 1.0, t_hat.data_ptr(),
+                                               rinv_t.data_ptr(), t_hi.data_ptr(), t_lo.data_ptr(), s), 'ssl_rows_normalize_f16x3(table)')
+        else:
+            check(lib.ssl_rows_normalize(table.ptr, table.stride, None, n, d, norm_mode, 1.0, t_hat.data_ptr(),
+                                         _ptr(t_t), rinv_t.data_ptr(), _ptr(t_hi), _ptr(t_lo), _ptr(t_thi), _ptr(t_tlo), npad, s),
+                  'ssl_rows_normalize(table)')
         with _timed('nce_gemm_fwd', dict(B=B, n=n, dim=d, tc=use_tc)):
-            if use_tc and live is not None:
+            if f16 and live is not None:
+                check(lib.ssl_softmax_gemm_f16x3_live(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), n, d, None, off,
+                                                      n_split, rs_part.data_ptr(), o_part.data_ptr(), live.data_ptr(), LIVE_ROWS, s),
+                      'ssl_softmax_gemm_f16x3_live(fwd)')
+            elif f16:
+                check(lib.ssl_softmax_gemm_f16x3(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), n, d, None, off,
+                                                 n_split, rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm_f16x3(fwd)')
+            elif use_tc and live is not None:
                 check(lib.ssl_softmax_gemm_tf32x3_live(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), t_thi.data_ptr(),
                                                        t_tlo.data_ptr(), npad, n, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(),
                                                        live.data_ptr(), LIVE_ROWS, s), 'ssl_softmax_gemm_tf32x3_live(fwd)')
@@ -817,10 +846,21 @@ def _nce_bwd(saved, g):
                       'ssl_nce_colscale_live')
             else:
                 check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), scale, colscale.data_ptr(), s), 'ssl_nce_colscale')
+            f16 = bool(tc) and tc[0].dtype == torch.float16
             n_split = choose_split((n + 127) // 128, ceil_to(B, 64) // 64, slots=NUM_SM if tc else 2 * NUM_SM, prefer_few=bool(tc))
             dt_part = torch.empty(n_split, n, d, **f)
             with _timed('nce_gemm_bwd', dict(B=B, n=n, dim=d, tc=bool(tc))):
-                if tc and live is not None:
+                if f16 and live is not None:
+                    a_hi, a_lo, _, _, t_hi, t_lo = tc
+                    check(lib.ssl_softmax_gemm_f16x3_live(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), B, d,
+                                                          colscale.data_ptr(), LOG2E / tau, n_split, None, dt_part.data_ptr(),
+                                                          live.data_ptr(), LIVE_COLS, s), 'ssl_softmax_gemm_f16x3_live(bwd)')
+                elif f16:
+                    a_hi, a_lo, _, _, t_hi, t_lo = tc
+                    check(lib.ssl_softmax_gemm_f16x3(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), B, d,
+                                                     colscale.data_ptr(), LOG2E / tau, n_split, None, dt_part.data_ptr(), s),
+                          'ssl_softmax_gemm_f16x3(bwd)')
+                elif tc and live is not None:
                     a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo = tc
                     check(lib.ssl_softmax_gemm_tf32x3_live(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), a_thi.data_ptr(),
                                                            a_tlo.data_ptr(), a_thi.shape[1], B, d, colscale.data_ptr(), LOG2E / tau, n_split, None,
@@ -955,14 +995,21 @@ def dense_logsumexp_mean(a: torch.Tensor, table: torch.Tensor, temp: float, eps:
 
 # ---- DirectAU: alignment / uniformity on unit rows (loss_utils.py:75-86) -----------------------------------
 
-def _unit_rows(e: Rows, idx, alpha: float, streamed: bool, use_tc: bool):
+def _unit_rows(e: Rows, idx, alpha: float, streamed: bool, use_tc: bool, f16: bool = False):
     """F.normalize of the gathered rows e[idx] (norm_mode 2), scaled by ``alpha``; with the operand copies the
-    contraction reads when asked (``streamed``: the C side needs the transposed copies as well)."""
+    contraction reads when asked (``streamed``: the C side needs the transposed copies as well, except for ``f16``, the
+    3xFP16 contraction, which reads the row-major fp16 hi / lo parts in both roles)."""
     dev, d, B = e.base.device, e.dim, idx.numel()
     Bp = ceil_to(B, 64)
     f = dict(device=dev, dtype=torch.float32)
     out, rinv = torch.empty(Bp, d, **f), torch.empty(B, **f)
     hi = lo = thi = tlo = out_t = None
+    if f16:
+        hi, lo = torch.empty(Bp, d, device=dev, dtype=torch.float16), torch.empty(Bp, d, device=dev, dtype=torch.float16)
+        with torch.cuda.device(dev):
+            check(lib.ssl_rows_normalize_f16x3(e.ptr, e.stride, idx.data_ptr(), B, d, 2, alpha, out.data_ptr(), rinv.data_ptr(),
+                                               hi.data_ptr(), lo.data_ptr(), _stream(e.base)), 'ssl_rows_normalize_f16x3(unit)')
+        return out, rinv, (hi, lo, thi, tlo, out_t)
     if use_tc:
         hi, lo = torch.empty(Bp, d, **f), torch.empty(Bp, d, **f)
         if streamed:
@@ -1024,14 +1071,18 @@ def _uniform_fwd(x: Rows, ix):
     # from 256 rows on the pair sum is >> e_ii, so removing e_ii loses little and the 3xTF32 contraction (1e-6) suffices
     use_tc = USE_TENSOR_CORES and d in (32, 64)
     off = 4.0 * LOG2E
-    r, _, (r_hi, r_lo, _, _, _) = _unit_rows(x, ix, off, False, use_tc)
-    c, rinv, (c_hi, c_lo, c_thi, c_tlo, c_t) = _unit_rows(x, ix, 1.0, True, use_tc)
+    f16 = use_tc and f16x3_applies(off)
+    r, _, (r_hi, r_lo, _, _, _) = _unit_rows(x, ix, off, False, use_tc, f16)
+    c, rinv, (c_hi, c_lo, c_thi, c_tlo, c_t) = _unit_rows(x, ix, 1.0, True, use_tc, f16)
     n_split = choose_split((B + 127) // 128, Bp // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
     rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
     with torch.cuda.device(dev):
         s = _stream(x.base)
         with _timed('nce_gemm_fwd', dict(B=B, n=B, dim=d, tc=use_tc)):
-            if use_tc:
+            if f16:
+                check(lib.ssl_softmax_gemm_f16x3(r_hi.data_ptr(), r_lo.data_ptr(), B, c_hi.data_ptr(), c_lo.data_ptr(), B, d, None, off,
+                                                 n_split, rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm_f16x3(uniformity)')
+            elif use_tc:
                 check(lib.ssl_softmax_gemm_tf32x3(r_hi.data_ptr(), r_lo.data_ptr(), B, c_hi.data_ptr(), c_lo.data_ptr(), c_thi.data_ptr(),
                                                   c_tlo.data_ptr(), Bp, B, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(), s),
                       'ssl_softmax_gemm_tf32x3(uniformity)')
