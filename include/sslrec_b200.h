@@ -415,7 +415,9 @@ SSL_API int ssl_unit_rows_bwd(const float *xhat, const float *rinv, const int64_
  * ssl_rowgemm   out[r, :n_out] (+)= leaky( scale * ( in1[r, :k1] M1 + in2[r, :k2] M2 ), slope )     row-local
  *     M1 [k1, n_out] row-major (m1_trans: given as [n_out, k1]); the second product is optional (in2 = NULL);
  *     pre_ref: in1[r, j] is multiplied by act'(pre_ref[r, j]) = (pre_ref > 0 ? 1 : pre_slope) while it is loaded
- *     (dZ = dY * act'(Y): LeakyReLU keeps the sign, so the saved OUTPUT tells the derivative); slope = 1: no activation.
+ *     (dZ = dY * act'(Y): with slope >= 0 LeakyReLU keeps the sign, so the saved OUTPUT tells the derivative; a negative
+ *     slope maps both branches to Y > 0 and would need the pre-activation, so engine.hyper_layer rejects it);
+ *     slope = 1: no activation.
  *     replaces  E_side @ W * mult (:43-44), adj @ hids (:106) and, in the backward, dZ @ lat^T + X @ dlat^T, H @ dlat, dA @ W^T.
  * ssl_colgemm   out[k1, k2] = post( scale * sum_r in1[r, :k1]^T (x) in2[r, :k2] )                   reduction over rows
  *     per-CTA partials part[ssl_colgemm_parts(n_rows), k1, k2] are reduced in a fixed order (bit-reproducible);
@@ -424,6 +426,8 @@ SSL_API int ssl_unit_rows_bwd(const float *xhat, const float *rinv, const int64_
  * ssl_hyper_dropout  F.dropout(A, p = 1 - keep) (:48-49): out = x * m / keep (accumulate: out += ..., the backward);
  *     mode 1: m = floor(U + keep) from the in-kernel counter-based generator keyed (seed, stream_id; row, 4-column group);
  *     mode 2: m = mask [n, h] fp32 of 0 / 1 (injected draws).
+ * n_rows = 0 (n = 0) is accepted with null row pointers (in1, in2, pre_ref, out; x, out, mask), as torch gives for an empty
+ *     side: ssl_rowgemm and ssl_hyper_dropout write nothing, ssl_colgemm writes out = 0 and out_act = leaky(0) = 0.
  * ------------------------------------------------------------------------------------------ */
 SSL_API int ssl_rowgemm(const float *in1, int64_t in1_stride, int32_t k1, const float *m1, int32_t m1_trans, const float *in2,
                 int64_t in2_stride, int32_t k2, const float *m2, int32_t m2_trans, const float *pre_ref, int64_t pre_stride,

@@ -14,7 +14,7 @@ import numpy as np
 M0, M1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57)
 W0, W1 = 0x9E3779B9, 0xBB67AE85
 MASK = np.uint64(0xFFFFFFFF)
-TAG_EDGE, TAG_NODE, TAG_NOISE, TAG_NEGS = 0x45444745, 0x4E4F4445, 0x4E4F4953, 0x4E454753
+TAG_EDGE, TAG_NODE, TAG_NOISE, TAG_NEGS, TAG_HYPR = 0x45444745, 0x4E4F4445, 0x4E4F4953, 0x4E454753, 0x48595052
 
 
 def philox4x32_10(c0, c1, c2, c3, seed: int):
@@ -53,6 +53,16 @@ def noise_uniform(seed: int, stream: int, n_rows: int, dim: int, row_offset: int
     quads = np.arange((dim + 3) // 4, dtype=np.uint64)[None, :]
     words = philox4x32_10(rows, quads, stream, TAG_NOISE, seed)
     return np.stack([u01(w) for w in words], axis=-1).reshape(n_rows, -1)[:, :dim]
+
+
+def hyper_keep(seed: int, stream: int, n: int, h: int, keep: float) -> np.ndarray:
+    """The [n, h] keep mask of HCCF's incidence dropout (hccf.py:48-49, ssl_hyper_dropout mode 1): element (r, 4q + t) is
+    kept when word t of the block keyed (r, q, stream, HYPR) gives floor(U + keep) == 1, evaluated in float32."""
+    rows = np.arange(n, dtype=np.uint64)[:, None]
+    quads = np.arange(h // 4, dtype=np.uint64)[None, :]
+    words = philox4x32_10(rows, quads, stream, TAG_HYPR, seed)
+    u = np.stack([u01(w) for w in words], axis=-1).reshape(n, h)
+    return (u + np.float32(keep)) >= np.float32(1.0)
 
 
 def sample_negs(users, trn_rowptr, trn_cols, n_item: int, seed: int, epoch: int) -> np.ndarray:

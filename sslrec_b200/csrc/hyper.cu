@@ -381,7 +381,8 @@ extern "C" int ssl_rowgemm(const float *in1, int64_t in1_stride, int32_t k1, con
                            int64_t in2_stride, int32_t k2, const float *m2, int32_t m2_trans, const float *pre_ref, int64_t pre_stride,
                            float pre_slope, float *out, int64_t out_stride, int32_t n_out, float scale, float slope, int32_t accumulate, int64_t n_rows,
                            void *stream) {
-    SSL_CHECK_ARG(in1 && m1 && out, "ssl_rowgemm: null argument");
+    // no rows: the row pointers may be null (torch gives an empty tensor data_ptr() == 0)
+    SSL_CHECK_ARG(n_rows >= 0 && m1 && (n_rows == 0 || (in1 && out)), "ssl_rowgemm: null argument or n_rows < 0");
     SSL_CHECK_ARG(ok_dim(k1) && (in2 == nullptr ? true : (ok_dim(k2) && m2 != nullptr)), "ssl_rowgemm: inner sizes out of range (4..128)");
     SSL_CHECK_ARG(ok_dim(n_out), "ssl_rowgemm: n_out %d out of range (4..128)", n_out);
     if (n_rows == 0) return SSL_OK;
@@ -406,7 +407,8 @@ extern "C" int ssl_colgemm_parts(int64_t n_rows) {
 extern "C" int ssl_colgemm(const float *in1, int64_t in1_stride, int32_t k1, const float *in2, int64_t in2_stride, int32_t k2,
                            const float *pre_ref, int64_t pre_stride, float slope, int64_t n_rows, float *part, float scale, int32_t mode,
                            const float *ref, float *out, float *out_act, void *stream) {
-    SSL_CHECK_ARG(in1 && in2 && part && out, "ssl_colgemm: null argument");
+    // no rows: in1 / in2 may be null; the one partial is zero, so out = 0 and out_act = leaky(0)
+    SSL_CHECK_ARG(n_rows >= 0 && part && out && (n_rows == 0 || (in1 && in2)), "ssl_colgemm: null argument or n_rows < 0");
     SSL_CHECK_ARG(ok_dim(k1) && ok_dim(k2), "ssl_colgemm: sizes %d x %d out of range (4..128)", k1, k2);
     SSL_CHECK_ARG(mode == 0 || (mode == 1 && ref != nullptr), "ssl_colgemm: mode 1 needs ref");
     const int grid = ssl_colgemm_parts(n_rows);
@@ -430,8 +432,10 @@ extern "C" int ssl_colgemm(const float *in1, int64_t in1_stride, int32_t k1, con
 
 static int hyper_dropout_launch(const float *x, float *out, int64_t n, int32_t h, float keep, int32_t mode, const float *mask, uint64_t seed,
                                 const uint64_t *seed_ptr, uint32_t stream_id, int32_t accumulate, void *stream) {
-    SSL_CHECK_ARG(x && out && h >= 4 && h % 4 == 0 && keep > 0.f && keep <= 1.f, "ssl_hyper_dropout: bad argument");
-    SSL_CHECK_ARG(mode == 1 || (mode == 2 && mask != nullptr), "ssl_hyper_dropout: mode 1 (in-kernel draw) or 2 (injected [n, h] float keep mask)");
+    // no rows: x, out and mask may be null
+    SSL_CHECK_ARG(n >= 0 && (n == 0 || (x && out)) && h >= 4 && h % 4 == 0 && keep > 0.f && keep <= 1.f, "ssl_hyper_dropout: bad argument");
+    SSL_CHECK_ARG(mode == 1 || (mode == 2 && (mask != nullptr || n == 0)),
+                  "ssl_hyper_dropout: mode 1 (in-kernel draw) or 2 (injected [n, h] float keep mask)");
     const int64_t total = n * (h / 4);
     if (total == 0) return SSL_OK;
     hyper_dropout_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, out, n, h, keep, mode, mask, seed, seed_ptr, stream_id, accumulate);

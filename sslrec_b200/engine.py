@@ -1404,6 +1404,10 @@ class _HyperLayerFn(torch.autograd.Function):
 
 
 def hyper_layer(x, a_u, a_i, slope: float, drop_u: HyperDrop, drop_i: HyperDrop) -> torch.Tensor:
+    # the backward takes act'(.) from the saved output (Y > 0 -> 1, else slope), which is right only while LeakyReLU keeps
+    # the sign; a negative slope would need the pre-activation saved as well
+    if not float(slope) >= 0.0:
+        raise ValueError(f'hyper_layer: LeakyReLU slope must be >= 0, got {slope}')
     return _HyperLayerFn.apply(x, a_u, a_i, float(slope), drop_u, drop_i)
 
 

@@ -539,10 +539,13 @@ def test_dense_logsumexp_mean_forward_backward(dim, B, n, use_tc, monkeypatch):
 
 
 @pytest.mark.parametrize('nu,ni,d,h,slope,keep', [(700, 500, 64, 128, 0.5, 0.5), (130, 65, 32, 16, 0.2, 1.0), (1000, 3, 48, 40, 1.0, 0.7),
-                                                  (64, 64, 128, 128, 0.5, 0.5)])
+                                                  (64, 64, 128, 128, 0.5, 0.5), (300, 200, 32, 128, 0.5, 0.5),
+                                                  (25500, 130, 64, 128, 1.0, 0.5)])
 def test_hyper_branch_forward_backward(nu, ni, d, h, slope, keep):
     """HCCF's hyper-graph layer (hccf.py:43-49, :100-108) on ssl_rowgemm / ssl_colgemm / ssl_hyper_dropout against torch
-    autograd in float64, with the dropout keeps injected."""
+    autograd in float64, with the dropout keeps injected.  d = 32, H = 128 is hccf.yml's shape (colgemm <8, 2> and <2, 8>);
+    25 500 user rows are more than 397 tiles of 64, so colgemm's CTAs sum two tiles each and the trailing ones are empty --
+    there at slope 1, where no LeakyReLU kink can flip a derivative and the tight tolerance holds."""
     from sslrec_b200 import engine as E
     g = torch.Generator().manual_seed(nu + d + h)
     eu, ei = torch.randn(nu, d, generator=g) * 0.3, torch.randn(ni, d, generator=g) * 0.3
@@ -589,6 +592,38 @@ def test_hyper_dropout_rng_keep_fraction_and_determinism():
     gacc = torch.zeros_like(a)
     E._drop(torch.full_like(a, 2.0), d, out=gacc, accumulate=True)
     assert torch.equal(gacc, 2.0 * o1)
+
+
+def test_hgnn_layer_one_side_forward_backward():
+    """HGNNLayer(leaky)(adj, embeds) = act(adj @ act(adj.T @ embeds)) (hccf.py:100-108) on its own: one side through
+    engine.hyper_layer, whose second side is empty (null row pointers), against torch autograd in float64."""
+    import torch.nn.functional as F
+    from sslrec_b200.general_cf.hccf import HGNNLayer
+    g = torch.Generator().manual_seed(17)
+    n, h, d, slope = 300, 40, 32, 0.5
+    adj, embeds, gy = torch.randn(n, h, generator=g) * 0.3, torch.randn(n, d, generator=g) * 0.5, torch.randn(n, d, generator=g)
+    a, e = adj.cuda().requires_grad_(True), embeds.cuda().requires_grad_(True)
+    y = HGNNLayer(slope)(a, e)
+    y.backward(gy.cuda())
+    a64, e64 = adj.double().requires_grad_(True), embeds.double().requires_grad_(True)
+    want = F.leaky_relu(a64 @ F.leaky_relu(a64.T @ e64, slope), slope)
+    want.backward(gy.double())
+    for name, got, ref in (('y', y.detach(), want.detach()), ('d adj', a.grad, a64.grad), ('d embeds', e.grad, e64.grad)):
+        H.close(got, ref, 2e-4, 2e-5 * ref.abs().max().item(), f'HGNNLayer {name}')
+
+
+def test_hyper_layer_rejects_a_negative_slope():
+    """The backward takes LeakyReLU's derivative from the saved output, which is right only while the activation keeps the
+    sign (slope >= 0); a negative slope is refused rather than trained with the wrong gradient."""
+    from sslrec_b200 import engine as E
+    from sslrec_b200.general_cf.hccf import HGNNLayer
+    g = torch.Generator().manual_seed(18)
+    x, a_u, a_i = torch.randn(50, 16, generator=g).cuda(), torch.randn(30, 8, generator=g).cuda(), torch.randn(20, 8, generator=g).cuda()
+    with pytest.raises(ValueError, match='slope'):
+        E.hyper_layer(x, a_u, a_i, -0.2, E.HyperDrop(), E.HyperDrop())
+    with pytest.raises(ValueError, match='slope'):
+        HGNNLayer(-0.2)(a_u, x[:30])
+    E.hyper_layer(x, a_u, a_i, 0.0, E.HyperDrop(), E.HyperDrop())          # slope 0 (ReLU) is fine
 
 
 @pytest.mark.parametrize('dim,V', [(64, 3), (128, 1)])
