@@ -159,6 +159,10 @@ typedef struct ssl_prop_args {
     const uint64_t *seed_ptr[SSL_MAX_VIEWS];  /* optional: the view's seed is READ FROM THE DEVICE (overrides seed[v]) -- a step captured
                                          in a CUDA graph draws fresh masks / noise at every replay because the host rewrites these
                                          words, not the launch arguments */
+    const uint32_t *row_bits[SSL_MAX_VIEWS];  /* optional per-view bitmap over the global rows (bit r of word r / 32; NULL = every
+                                         row): a view whose bit is clear for a row gathers nothing there and stores nothing.
+                                         Only a launch that writes sum_out without x_out and without reduce_views may restrict
+                                         a view (the last summed layer, read by the losses at batch rows only) */
 } ssl_prop_args;
 
 SSL_API int ssl_propagate_layer(const ssl_plan *plan, const ssl_prop_args *args, void *stream);
@@ -325,6 +329,9 @@ SSL_API int ssl_nce_colscale_live(const float *rowsum, int64_t batch, const int6
  * the result does not depend on scheduling.
  * ------------------------------------------------------------------------------------------ */
 SSL_API int ssl_unique_ids_scratch(int64_t n_range, int64_t *words);
+/* bits[0, ceil(n_range / 32)) = the bitmap of the ids idx[0, n) in [0, n_range) (ids outside are ignored): the row_bits of
+ * ssl_prop_args built on the device, with no host read (CUDA-graph safe) */
+SSL_API int ssl_row_bitmap(const int64_t *idx, int64_t n, int64_t n_range, uint32_t *bits, int64_t n_words, void *stream);
 SSL_API int ssl_unique_ids(const int64_t *idx, int64_t n, int64_t n_range, uint32_t *scratch, int64_t scratch_n_words,
                    int64_t *out, int64_t *count, void *stream);
 

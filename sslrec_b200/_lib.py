@@ -37,7 +37,7 @@ class PropArgs(C.Structure):
         ('noise_eps', C.c_float), ('seed', C.c_uint64 * MAX_VIEWS),
         ('edge_stream_id', C.c_uint32), ('noise_stream_id', C.c_uint32),
         ('n_peers', C.c_int32), ('x_out_peers', vp * MAX_PEERS), ('sum_out_peers', vp * MAX_PEERS),
-        ('reg_coef_dev', vp), ('reg_src2', vp), ('seed_ptr', vp * MAX_VIEWS),
+        ('reg_coef_dev', vp), ('reg_src2', vp), ('seed_ptr', vp * MAX_VIEWS), ('row_bits', vp * MAX_VIEWS),
     ]
 
 
@@ -84,6 +84,7 @@ def _load():
         'ssl_nce_colscale_live': (C.c_int, [vp, i64, vp, vp, f32, vp, vp]),
         'ssl_unique_ids_scratch': (C.c_int, [i64, c_i64p]),
         'ssl_unique_ids': (C.c_int, [vp, i64, i64, vp, i64, vp, vp, vp]),
+        'ssl_row_bitmap': (C.c_int, [vp, i64, i64, vp, i64, vp]),
         'ssl_sumsq': (C.c_int, [vp, i64, vp, vp]),
         'ssl_sum': (C.c_int, [vp, i64, f32, vp, vp]),
         'ssl_axpy': (C.c_int, [vp, vp, i64, vp, f32, vp]),

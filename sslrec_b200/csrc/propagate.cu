@@ -92,6 +92,17 @@ __device__ __forceinline__ void prop_item(const PlanDev &p, const ssl_prop_args 
     const int r = it.x;
     const uint32_t grow = (uint32_t)r + ((r < p.split_local) ? p.off_a : p.off_b);    // global row
 
+    // row-restricted views (row_bits): decided once per item; an inactive view issues no gathers (its partial stays zero)
+    // and stores nothing.  At active rows the arithmetic and its order are those of an unrestricted launch.
+    uint32_t act = 0u;                 // bit vi: view vbase + vi is computed at this row
+#pragma unroll
+    for (int vi = 0; vi < V; ++vi) {
+        const uint32_t *bits = a.row_bits[vbase + vi];
+        if (bits == nullptr || (r >= 0 && ((__ldg(bits + (grow >> 5)) >> (grow & 31)) & 1u) != 0u)) act |= 1u << vi;
+    }
+    // accumulators that gather: per view, or -- one shared accumulator -- when any view is computed; 0 on idle lanes
+    const uint32_t gather = lane_on ? (SHARED ? (act != 0u ? 1u : 0u) : act) : 0u;
+
     float4 acc[NA];
 #pragma unroll
     for (int v = 0; v < NA; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -137,7 +148,7 @@ __device__ __forceinline__ void prop_item(const PlanDev &p, const ssl_prop_args 
 #pragma unroll
                 for (int v = 0; v < NA; ++v) {
                     x[u][v] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (lane_on && wj[u][NW == 1 ? 0 : v] != 0.f) x[u][v] = ssl::ldg4(xr + ((VM || a.in_views == 1) ? 0 : v * dim));
+                    if (((gather >> v) & 1u) && wj[u][NW == 1 ? 0 : v] != 0.f) x[u][v] = ssl::ldg4(xr + ((VM || a.in_views == 1) ? 0 : v * dim));
                 }
             }
 #pragma unroll
@@ -182,6 +193,7 @@ __device__ __forceinline__ void prop_item(const PlanDev &p, const ssl_prop_args 
     const size_t out_row = (size_t)grow * nv * dim;
 #pragma unroll
     for (int vi = 0; vi < V; ++vi) {
+        if (!((act >> vi) & 1u)) continue;            // the whole group skips (one row per group): the noise shuffle stays convergent
         const int v = vbase + vi;
         float4 x = acc[SHARED ? 0 : vi];
         if (a.residual != nullptr && lane_on) ssl::add4(x, ssl::ldg4(a.residual + out_row + v * dim + col));
@@ -431,6 +443,9 @@ extern "C" int ssl_propagate_layer(const ssl_plan *plan, const ssl_prop_args *ar
     SSL_CHECK_ARG(a.n_sum_src >= 0 && a.n_sum_src <= SSL_MAX_SUM_SRC, "ssl_propagate_layer: n_sum_src out of range");
     SSL_CHECK_ARG((a.reg_src == nullptr && a.reg_src2 == nullptr) || a.reduce_views, "ssl_propagate_layer: reg_src / reg_src2 need reduce_views");
     SSL_CHECK_ARG(a.reg_coef_dev == nullptr || a.reg_src != nullptr, "ssl_propagate_layer: reg_coef_dev without reg_src");
+    for (int v = 0; v < a.n_views; ++v)
+        SSL_CHECK_ARG(a.row_bits[v] == nullptr || (a.sum_out != nullptr && a.x_out == nullptr && !a.reduce_views),
+                      "ssl_propagate_layer: a row-restricted view (row_bits[%d]) needs a launch that writes sum_out only, without x_out or reduce_views", v);
     bool any_edge = false;
     for (int v = 0; v < a.n_views; ++v) {
         SSL_CHECK_ARG(a.edge_mode[v] >= 0 && a.edge_mode[v] <= 2 && a.noise_mode[v] >= 0 && a.noise_mode[v] <= 2, "ssl_propagate_layer: bad mode for view %d", v);

@@ -180,3 +180,18 @@ extern "C" int ssl_unique_ids(const int64_t *idx, int64_t n, int64_t n_range, ui
     SSL_LAUNCH_CHECK("compact_kernel");
     return SSL_OK;
 }
+
+extern "C" int ssl_row_bitmap(const int64_t *idx, int64_t n, int64_t n_range, uint32_t *bits, int64_t n_words, void *stream) {
+    SSL_CHECK_ARG(bits && (idx || n == 0), "ssl_row_bitmap: null argument");
+    SSL_CHECK_ARG(n >= 0 && n_range >= 1, "ssl_row_bitmap: bad sizes");
+    SSL_CHECK_ARG(n_words >= (n_range + 31) / 32, "ssl_row_bitmap: %lld words, %lld needed", (long long)n_words, (long long)((n_range + 31) / 32));
+    const unsigned grid_clear = (unsigned)std::max<int64_t>(1, std::min<int64_t>((n_words + kThreads - 1) / kThreads, 4 * ssl::kNumSM));
+    clear_kernel<<<grid_clear, kThreads, 0, STREAM>>>(bits, n_words);
+    SSL_LAUNCH_CHECK("clear_kernel");
+    if (n > 0) {
+        const unsigned grid_mark = (unsigned)std::min<int64_t>((n + kThreads - 1) / kThreads, 8 * ssl::kNumSM);
+        mark_kernel<<<grid_mark, kThreads, 0, STREAM>>>(idx, n, n_range, bits);
+        SSL_LAUNCH_CHECK("mark_kernel");
+    }
+    return SSL_OK;
+}

@@ -127,6 +127,7 @@ class ViewSpec:
     node_keep: float = 1.0
     node_mask: Optional[torch.Tensor] = None
     seed: int = 0
+    row_bits: Optional[torch.Tensor] = None   # ``row_bitmap``: the losses read this view of the layer sum at these rows only
 
     def edge_mask_for(self, layer: int) -> Optional[torch.Tensor]:
         if self.edge_mode != 2:
@@ -215,21 +216,42 @@ class SeedStream:
 
 class Rows:
     """Reference to the rows [off, off+n) of view ``v`` of a [*, V, d] (or [*, d]) fp32 tensor, plus
-    where their gradient goes (a sink of the same shape, created zeroed on first use)."""
+    where their gradient goes: a sink created zeroed on first use, either of the same shape or -- ``grad_views`` = 1, a
+    view-linear propagation (``Propagation.view_linear``) -- one [*, 1, d] sink that every view's gradient is added to."""
 
     def __init__(self, base: torch.Tensor, v: int, n_views: int, off: int, n: int, dim: int,
-                 sink_get=None, token: Optional[torch.Tensor] = None, comm=None):
+                 sink_get=None, token: Optional[torch.Tensor] = None, comm=None, grad_views: Optional[int] = None,
+                 restricted: bool = False):
         self.base, self.v, self.n_views, self.off, self.n, self.dim = base, v, n_views, off, n, dim
+        self.restricted = restricted    # the view was computed at its marked rows only: gather it by index, never whole
         self.sink_get, self.token = sink_get, token
         self.comm = comm          # RowShard: as a *table* operand only the rank's own rows are contracted
+        self.grad_views = n_views if grad_views is None else grad_views
+        if self.grad_views not in (1, n_views):
+            raise ValueError('a sink holds every view or one summed view')
 
     def sub(self, lo: int, hi: int) -> 'Rows':
         """The same reference restricted to global rows [lo, hi) of the underlying tensor."""
-        return Rows(self.base, self.v, self.n_views, lo, hi - lo, self.dim, self.sink_get, self.token)
+        return Rows(self.base, self.v, self.n_views, lo, hi - lo, self.dim, self.sink_get, self.token, grad_views=self.grad_views,
+                    restricted=self.restricted)
+
+    def require_whole(self, what: str) -> None:
+        if self.restricted:
+            raise RuntimeError(f'sslrec_b200: view {self.v} of this layer sum was computed at the rows its ViewSpec.row_bits marks '
+                               f'only; {what} reads every row')
 
     @property
     def stride(self) -> int:
         return self.n_views * self.dim
+
+    @property
+    def grad_stride(self) -> int:
+        """Row stride of the gradient sink (elements): ``stride``, or ``dim`` when the views share one sink."""
+        return self.grad_views * self.dim
+
+    @property
+    def _grad_v(self) -> int:
+        return self.v if self.grad_views == self.n_views else 0
 
     @property
     def ptr(self) -> int:
@@ -239,10 +261,16 @@ class Rows:
         if self.sink_get is None:
             return None
         g = self.sink_get()
-        return g.data_ptr() + 4 * ((self.off * self.n_views + self.v) * self.dim)
+        return g.data_ptr() + 4 * ((self.off * self.grad_views + self._grad_v) * self.dim)
+
+    def grad_dense(self) -> torch.Tensor:
+        """A strided torch view of the referenced rows' gradient in the sink."""
+        g = self.sink_get().view(-1, self.grad_views, self.dim)
+        return g[self.off:self.off + self.n, self._grad_v, :]
 
     def dense(self) -> torch.Tensor:
         """A strided torch view of the referenced rows (for inspection / tests)."""
+        self.require_whole('Rows.dense()')
         b = self.base.view(-1, self.n_views, self.dim)
         return b[self.off:self.off + self.n, self.v, :]
 
@@ -266,18 +294,23 @@ class PropState:
         self._g_layers: Dict[int, torch.Tensor] = {}
         self._g_e0 = None
         self.reg_pending: Optional[torch.Tensor] = None     # upstream gradient of sum ||E0||^2 (device scalar), folded into the last backward launch
+        self.grad_views = 1 if prop.view_linear else self.n_views     # views of the E / layer sinks (1: every view's gradient summed)
+        self.restricted_views = set()    # views of E computed at their row_bits rows only (Propagation.forward)
 
     # ---- sinks -------------------------------------------------------------------------------
+    def _sink(self, like: torch.Tensor) -> torch.Tensor:
+        return torch.zeros(like.shape[0], self.grad_views, self.dim, device=like.device, dtype=torch.float32)
+
     def g_sum(self) -> torch.Tensor:
         if self._g_sum is None:
-            self._g_sum = torch.zeros_like(self.E)
+            self._g_sum = self._sink(self.E)
         return self._g_sum
 
     def g_layer(self, k: int) -> torch.Tensor:
         if k == 0:
             return self.g_e0()
         if k not in self._g_layers:
-            self._g_layers[k] = torch.zeros_like(self.layers[k])
+            self._g_layers[k] = self._sink(self.layers[k])
         return self._g_layers[k]
 
     def g_e0(self) -> torch.Tensor:
@@ -289,11 +322,12 @@ class PropState:
     def _rows(self, which, v: int, off: int, n: int) -> Rows:
         comm = self.prop.loss_comm
         if which == 'sum':
-            return Rows(self.E, v, self.n_views, off, n, self.dim, self.g_sum, self.token, comm)
+            return Rows(self.E, v, self.n_views, off, n, self.dim, self.g_sum, self.token, comm, self.grad_views,
+                        restricted=v in self.restricted_views)
         k = int(which)
         if k == 0:           # layer 0 is E0 itself (ncl.py:75)
             return Rows(self.e0, 0, 1, off, n, self.dim, self.g_e0, self.token, comm)
-        return Rows(self.layers[k], v, self.n_views, off, n, self.dim, lambda: self.g_layer(k), self.token, comm)
+        return Rows(self.layers[k], v, self.n_views, off, n, self.dim, lambda: self.g_layer(k), self.token, comm, self.grad_views)
 
     def users(self, v: int = 0, which='sum') -> Rows:
         return self._rows(which, v, 0, self.n_user)
@@ -328,6 +362,10 @@ class Propagation:
         if self.sum_layers > self.n_layers or self.sum_layers + 1 > _lib.MAX_SUM_SRC + 1:
             raise ValueError('sum_layers out of range')
         self.any_node = any(v.node_mode != 0 for v in self.views)
+        # view-linear: every view's layers are the same linear map Â (no edge mask, no node drop).  The views then differ only
+        # by the SimGCL perturbation eps sign(x) û, whose derivative is zero, so the transposed recursions of all views can be
+        # summed before they run -- one [N, 1, d] sink and one-view backward launches instead of V of each
+        self.view_linear = all(v.edge_mode == 0 and v.node_mode == 0 for v in self.views)
 
     # ---- argument block ------------------------------------------------------------------------
     def _args(self, dim: int, layer: int, transpose: bool) -> PropArgs:
@@ -356,12 +394,28 @@ class Propagation:
         meta = None
         if TIMER is not None:
             shared = a.in_views == 1 and not any(a.edge_mode[i] for i in range(a.n_views))
-            meta = dict(views=a.n_views, gather_views=1 if shared else a.n_views, dim=a.dim, residual=bool(a.residual), reg_src2=bool(a.reg_src2),
+            gather = 1 if shared else a.n_views
+            restricted = [i for i in range(a.n_views) if a.row_bits[i]]
+            if restricted and not shared and not torch.cuda.is_current_stream_capturing():
+                # a restricted view gathers the stored entries of its marked rows only (host read: timed runs only)
+                gather -= sum(1.0 - self._marked_entry_fraction(self.views[i].row_bits) for i in restricted)
+            meta = dict(views=a.n_views, gather_views=gather, restricted_views=len(restricted), dim=a.dim, residual=bool(a.residual), reg_src2=bool(a.reg_src2),
                         x_out=bool(a.x_out), sum_out=bool(a.sum_out), reduce_views=bool(a.reduce_views),
                         sum_src=[a.sum_src_views[i] for i in range(a.n_sum_src)], reg_src=bool(a.reg_src),
                         nnz=self.plan.nnz, rows=self.plan.n_rows)
         with torch.cuda.device(ref.device), _timed(name, meta):
             check(lib.ssl_propagate_layer(self.plan.handle, C.byref(a), _stream(ref)), 'ssl_propagate_layer')
+
+    def _marked_entry_fraction(self, bits: torch.Tensor) -> float:
+        """Share of the plan's stored entries that lie in the rows a row bitmap marks."""
+        plan = self.plan
+        deg = getattr(plan, '_deg_dev', None)
+        if deg is None or deg.device != bits.device:
+            deg = torch.from_numpy(plan.h_rowptr.astype('int64')).diff().to(bits.device)
+            plan._deg_dev = deg
+        rows = torch.arange(deg.numel(), device=bits.device)
+        marked = (bits.to(torch.int64)[rows >> 5] >> (rows & 31)) & 1
+        return float((deg * marked).sum().item()) / max(1, plan.nnz)
 
     def _node_drop(self, x: torch.Tensor, out: torch.Tensor, backward: bool):
         V = len(self.views)
@@ -450,6 +504,13 @@ class Propagation:
             if k == self.sum_layers:
                 st.E, e_tb = self._out('E', (N, V, d), e0)
                 a.sum_out = st.E.data_ptr()
+                if not need_out and self.comm is None:
+                    # views the losses read at batch rows only: gathered and written at the marked rows (the kernel accepts a
+                    # restriction only for a launch that writes sum_out alone; a row-sharded launch computes every row)
+                    for i, v in enumerate(self.views):
+                        if v.row_bits is not None:
+                            a.row_bits[i] = v.row_bits.data_ptr()
+                            st.restricted_views.add(i)
                 self._set_peers(a, 'sum_out_peers', e_tb)
                 a.n_sum_src = len(srcs)
                 for i, (s, sv) in enumerate(srcs):
@@ -468,9 +529,11 @@ class Propagation:
     # ---- backward ------------------------------------------------------------------------------
     def backward(self, st: PropState) -> torch.Tensor:
         """Consumes the sinks of ``st``; returns dE0 [N, d].  Row-sharded: only the rows this rank owns are computed
-        (the others are zero) -- the sharded Adam updates exactly those and stores them to the peers."""
+        (the others are zero) -- the sharded Adam updates exactly those and stores them to the peers.
+
+        View-linear: the sinks hold sum_v G^v, and D_{k-1} = Â^T D_k + sum_v G^v_{k-1} runs as one view."""
         e0 = st.e0
-        N, d, V = st.n, st.dim, st.n_views
+        N, d, V = st.n, st.dim, st.grad_views
         opts = dict(device=e0.device, dtype=torch.float32)
         L, S = self.n_layers, self.sum_layers
 
@@ -506,7 +569,7 @@ class Propagation:
         D = residual(top)
         for k in range(top, 0, -1):           # D_{k-1} = A_v^T D_k + residual(k-1)
             a = self._args(d, k, transpose=True)
-            a.in_views = V
+            a.n_views = a.in_views = V
             a.x_in = D.data_ptr()
             res = residual(k - 1)
             if res is not None:
@@ -671,7 +734,7 @@ def _bpr_bwd(users: Rows, items: Rows, ancs, poss, negs, coef, g):
     with torch.cuda.device(g.device):
         check(lib.ssl_bpr_bwd(users.ptr, users.stride, items.ptr, items.stride, ancs.data_ptr(), poss.data_ptr(),
                               negs.data_ptr(), ancs.numel(), users.dim, coef.data_ptr(), g.data_ptr(), 1.0,
-                              users.grad_ptr(), users.stride, items.grad_ptr(), items.stride, _stream(g)), 'ssl_bpr_bwd')
+                              users.grad_ptr(), users.grad_stride, items.grad_ptr(), items.grad_stride, _stream(g)), 'ssl_bpr_bwd')
 
 
 class _BprFn(torch.autograd.Function):
@@ -726,6 +789,7 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
     """``live``: optional int64 DEVICE scalar; only the first ``*live`` of the ``idx`` rows are anchors (a padded list of
     capacity idx.numel(), see ``dense_infonce_spec_nodes_mean_dev``).  Shapes and n_split then depend on the capacity only."""
     dev = table.base.device
+    table.require_whole('an InfoNCE table operand')
     d = table.dim
     B, n = idx.numel(), table.n
     Bp, npad = ceil_to(B, 64), ceil_to(n, 64)
@@ -826,18 +890,18 @@ def _nce_bwd(saved, g):
     with torch.cuda.device(dev):
         s = _stream(g)
         g1, g2, gt = e1.grad_ptr(), e2.grad_ptr(), table.grad_ptr()
-        gt_stride, local_dt = table.stride, None
+        gt_stride, local_dt = table.grad_stride, None
         if comm is not None and gt is not None:
             # own rows' dense gradient goes to a compact block that is all-gathered and added to the sink
             local_dt = torch.zeros(comm.side_block(full_table.n), d, **f)
             gt, gt_stride = local_dt.data_ptr(), d
         if live is not None and (g1 is not None or g2 is not None):        # rows b < live only, mean over live
             check(lib.ssl_nce_bwd_rows_live(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
-                                            idx.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, g1, e1.stride, g2, e2.stride, s),
+                                            idx.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, g1, e1.grad_stride, g2, e2.grad_stride, s),
                   'ssl_nce_bwd_rows_live')
         elif g1 is not None or g2 is not None:
             check(lib.ssl_nce_bwd_rows(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
-                                       idx.data_ptr(), B, d, tau, g.data_ptr(), scale, g1, e1.stride, g2, e2.stride, s),
+                                       idx.data_ptr(), B, d, tau, g.data_ptr(), scale, g1, e1.grad_stride, g2, e2.grad_stride, s),
                   'ssl_nce_bwd_rows')
         if gt is not None and n > 0:
             colscale = torch.zeros(ceil_to(B, 64), **f)   # padded tail is read (then masked) by the tile loads
@@ -882,8 +946,7 @@ def _nce_bwd(saved, g):
                                         gt_stride, 1, s), 'ssl_nce_bwd_table')
         if local_dt is not None:
             dense = comm.allgather_side(local_dt, full_table.n)
-            sink = full_table.sink_get().view(-1, full_table.n_views, d)
-            sink[full_table.off:full_table.off + full_table.n, full_table.v, :] += dense
+            full_table.grad_dense().add_(dense)
 
 
 class _InfoNceFn(torch.autograd.Function):
@@ -1046,7 +1109,7 @@ def _align_bwd(pack, g):
             gp = rows.grad_ptr()
             if gp is not None:
                 check(lib.ssl_unit_rows_bwd(a.data_ptr(), ri.data_ptr(), idx.data_ptr(), B, d, a.data_ptr(), c, b.data_ptr(), -c,
-                                            g.data_ptr(), 1.0, gp, rows.stride, s), 'ssl_unit_rows_bwd(align)')
+                                            g.data_ptr(), 1.0, gp, rows.grad_stride, s), 'ssl_unit_rows_bwd(align)')
 
 
 def _uniform_fwd(x: Rows, ix):
@@ -1104,7 +1167,7 @@ def _uniform_bwd(pack, g):
     coef = (g * 8.0 / total).contiguous()                       # d total / d x^_i = 8 sum_{j != i} e_ij x^_j
     with torch.cuda.device(g.device):
         check(lib.ssl_unit_rows_bwd(c.data_ptr(), rinv.data_ptr(), ix.data_ptr(), ix.numel(), x.dim, w.data_ptr(), 1.0, None, 0.0,
-                                    coef.data_ptr(), 1.0, gp, x.stride, _stream(g)), 'ssl_unit_rows_bwd(uniformity)')
+                                    coef.data_ptr(), 1.0, gp, x.grad_stride, _stream(g)), 'ssl_unit_rows_bwd(uniformity)')
 
 
 class _AlignFn(torch.autograd.Function):
@@ -1269,6 +1332,18 @@ def unique_ids(idx: torch.Tensor, n_range: int):
         check(lib.ssl_unique_ids(idx.data_ptr(), idx.numel(), int(n_range), scratch.data_ptr(), words.value, out.data_ptr(),
                                  count.data_ptr(), _stream(idx)), 'ssl_unique_ids')
     return out, count
+
+
+def row_bitmap(n_rows: int, device, *index_lists) -> torch.Tensor:
+    """uint32 bitmap over [0, n_rows) marking every id of ``index_lists`` (pairs (ids, offset): marks ids + offset), built on
+    ``device`` with no host read (``ssl_row_bitmap``): ``ViewSpec.row_bits`` of a view the losses read at batch rows only."""
+    dev = torch.device(device)
+    idx = torch.cat([_i64(ids, dev).reshape(-1) + int(off) for ids, off in index_lists])
+    n_words = (int(n_rows) + 31) // 32
+    bits = torch.empty(n_words, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ssl_row_bitmap(idx.data_ptr(), idx.numel(), int(n_rows), bits.data_ptr(), n_words, _stream(idx)), 'ssl_row_bitmap')
+    return bits
 
 
 def dense_infonce_spec_nodes_mean_dev(embeds1, embeds2, ids, temp):
