@@ -49,6 +49,218 @@ def gpu_injection(model_key, case, hp, adj, dr, device='cuda'):
     return inj
 
 
+# ---- model-level cases off the golden shapes (tests/test_gpu_model_paths.py, tests/test_host_model_paths.py) -------------------
+
+# hyper-parameters of each drop-in model: the goldens' (the YAML values, with BASELINE.json's layer counts)
+PATH_HP_FROM = {'lightgcn': ('lightgcn', 'small'), 'simgcl': ('simgcl', 'small'), 'sgl': ('sgl', 'small'), 'sgl_nd': ('sgl_nd', 'tiny'),
+                'ncl': ('ncl_k50', 'small'), 'hccf': ('hccf_h128', 'small'), 'directau': ('directau', 'small'),
+                'lightgcl': ('lightgcl', 'small')}
+PATH_USERS, PATH_ITEMS, PATH_EDGES = 600, 450, 5000
+HUB_USER, HUB_ITEM = 0, 0
+HUB_USER_DEG, HUB_ITEM_MIN_DEG = 160, 320         # a split row on each side of side_split (rows of > 128 entries are split)
+LOSS_RTOL, GRAD_RTOL, GRAD_MAXTOL, PRED_RTOL = 1e-5, 2e-4, 5e-6, 1e-5
+KINK_MARGIN = 1e-6
+
+
+def _path_matrix():
+    """(model_key, embedding_size, temperature or None, batch, hyper_num or None) of every model-level path case."""
+    out = []
+    for d in (16, 20, 48, 128):              # the FP32-FMA contraction; propagation G = 4, 8 (idle lanes), 16 (idle lanes), 32
+        out.append(('lightgcn', d, None, 300, None))
+        out += [(m, d, 0.2, 300, None) for m in ('simgcl', 'sgl', 'sgl_nd', 'ncl', 'hccf', 'lightgcl')]
+        out += [('directau', d, None, 300, None), ('directau', d, None, 100, None)]     # contraction / pairwise uniformity
+    out += [('lightgcn', 4, None, 300, None), ('simgcl', 4, 0.2, 300, None)]          # propagation G = 1
+    # 3xTF32 InfoNCE.  Not SGL: with its cl_weight of 1 the two edge-dropped views of a hub row nearly coincide, the softmax
+    # of its anchor row sits almost all on the positive, and below tau ~ 0.09 even a float32 evaluation of the loss misses the
+    # gradient bound by 4-50x against float64 (the per-row gradient is a small difference of O(1 / tau) terms)
+    out += [(m, d, 0.05, 300, None) for d in (32, 64) for m in ('simgcl', 'ncl', 'hccf')]
+    out += [('simgcl', 64, 0.0900, 300, None), ('simgcl', 64, 0.0905, 300, None)]     # either side of the 3xFP16 offset bound
+    out += [('hccf', 20, 0.2, 300, 16), ('hccf', 48, 0.2, 300, 40)]                   # hyper branch at other (d, H)
+    return out
+
+
+PATH_CASES = _path_matrix()
+# cases whose default seed puts a kink input within KINK_MARGIN of its |term| sum (kink_margin): the first later seed that does not
+PATH_SEEDS = {('simgcl', 128, 0.2): 43, ('hccf', 128, 0.2): 42, ('hccf', 64, 0.05): 43}
+
+
+def path_case_id(case):
+    m, d, tau, b, h = case
+    return f'{m}-d{d}' + ('' if tau is None else f'-tau{tau}') + f'-b{b}' + ('' if h is None else f'-h{h}')
+
+
+def path_setup(model_key, dim, tau, batch, hyper_num):
+    """-> case, hp, adjacency, draws and injected state of one path case."""
+    case = path_case(dim, batch, PATH_SEEDS.get((model_key, dim, tau), 41))
+    hp = path_hp(model_key, dim, tau, hyper_num)
+    adj = O.normalized_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
+    dr = replay.draws(model_key, case, hp, adj)
+    return case, hp, adj, dr, path_state(model_key, case, hp, adj, dr)
+
+
+def path_hp(model_key, dim, tau=None, hyper_num=None):
+    hp = dict(replay.load_golden(*PATH_HP_FROM[model_key])['hp'])
+    hp['embedding_size'] = dim
+    if tau is not None:
+        hp['temp' if model_key == 'lightgcl' else 'temperature'] = tau
+    if hyper_num is not None:
+        hp['hyper_num'] = hyper_num
+    return hp
+
+
+def path_case(dim, batch=300, seed=41):
+    """A ``inputs.make_case``-shaped case of 600 users x 450 items: the skewed graph of ``inputs.bipartite_edges`` (its last
+    users / items are isolated), a user hub of degree 160 and an item hub of degree >= 320, and a batch of ``batch`` edges with
+    repeated anchors, both hubs and an isolated item among the negatives."""
+    U, I = PATH_USERS, PATH_ITEMS
+    rows, cols = inputs.bipartite_edges(U, I, PATH_EDGES, seed)
+    rs = np.random.RandomState(seed + 1000)
+    live_u, live_i = U - U // 40, I - I // 40
+    pairs = {(u, i) for u, i in zip(rows.tolist(), cols.tolist()) if u != HUB_USER}
+    pairs |= {(HUB_USER, int(i)) for i in rs.choice(live_i, HUB_USER_DEG, replace=False)}
+    for u in rs.permutation(live_u).tolist():
+        if sum(1 for p in pairs if p[1] == HUB_ITEM) >= HUB_ITEM_MIN_DEG:
+            break
+        pairs.add((u, HUB_ITEM))
+    pairs = np.array(sorted(pairs), dtype=np.int64)[rs.permutation(len(pairs))]
+    rows, cols = pairs[:, 0].copy(), pairs[:, 1].copy()
+    g = torch.Generator().manual_seed(seed + 2000)
+    a, b = float(np.sqrt(6.0 / (U + dim))), float(np.sqrt(6.0 / (I + dim)))
+    user_e = (torch.rand(U, dim, generator=g) * 2 - 1) * a
+    item_e = (torch.rand(I, dim, generator=g) * 2 - 1) * b
+    pick = rs.randint(0, len(rows), size=batch)
+    pick[:3] = np.flatnonzero(rows == HUB_USER)[:3]         # the user hub, three times
+    pick[3:6] = np.flatnonzero(cols == HUB_ITEM)[:3]        # the item hub as a positive
+    ancs, poss = rows[pick].copy(), cols[pick].copy()
+    negs = rs.randint(0, I, size=batch).astype(np.int64)
+    negs[0], negs[1] = HUB_ITEM, I - 1                      # the item hub and an isolated item as negatives
+    return dict(name=f'paths_d{dim}_b{batch}', n_user=U, n_item=I, dim=dim, batch=batch, seed=seed,
+                rows=rows, cols=cols, user_e=user_e, item_e=item_e, ancs=ancs, poss=poss, negs=negs)
+
+
+def path_state(model_key, case, hp, adj, dr):
+    """The state both sides are given besides the draws: NCL's k-means (float64 Lloyd iterations from the drawn initial
+    centroids, rounded to float32) and LightGCL's SVD factors (a seeded ``torch.svd_lowrank`` of its adjacency, float32),
+    in the keys ``replay.oracle_loss`` reads from its ``golden`` argument."""
+    name = model_key.split('_')[0]
+    st = {}
+    if name == 'ncl':
+        for side, e in (('user', case['user_e']), ('item', case['item_e'])):
+            cents, idx, _ = O.kmeans(e.double(), dr[f'init_{side}_centroids'].double(), iters=100)
+            st[f'{side}_centroids'] = cents.float().numpy()
+            st[f'{side}2cluster'] = idx.numpy()
+    elif name == 'lightgcl':
+        ladj = O.lightgcl_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
+        up = ladj.rows < ladj.n_user
+        m = torch.sparse_coo_tensor(torch.from_numpy(np.vstack([ladj.rows[up], ladj.cols[up] - ladj.n_user])),
+                                    torch.from_numpy(ladj.vals[up]).double(), (ladj.n_user, ladj.n_item)).coalesce()
+        with torch.random.fork_rng():
+            torch.manual_seed(case['seed'])
+            u, s, v = torch.svd_lowrank(m, q=hp['svd_q'])
+        st['svd_ut'], st['svd_vt'] = u.T.contiguous().float().numpy(), v.T.contiguous().float().numpy()
+        st['svd_u_mul_s'], st['svd_v_mul_s'] = (u * s).float().numpy(), (v * s).float().numpy()
+    return st
+
+
+def path_params(model_key, case, dr, dtype):
+    params = {'user_embeds': case['user_e'], 'item_embeds': case['item_e']}
+    if 'user_w' in dr:
+        params['user_hyper_embeds'], params['item_hyper_embeds'] = dr['user_w'], dr['item_w']
+    for i, w in enumerate(dr.get('ws', [])):
+        params[f'Ws.{i}.W'] = w
+    return {k: v.to(dtype).clone().requires_grad_(True) for k, v in params.items()}
+
+
+def pred_users_mask(case, n=64):
+    bt = min(n, case['n_user'])
+    mask = torch.zeros(bt, case['n_item'], dtype=torch.int64)
+    sel = case['rows'] < bt
+    mask[torch.from_numpy(case['rows'][sel]), torch.from_numpy(case['cols'][sel])] = 1
+    return torch.arange(bt), mask
+
+
+def path_oracle(model_key, case, hp, adj, dr, st, dtype=torch.float64):
+    """cal_loss, backward and full_predict of the oracle in ``dtype`` -> dict(loss, parts, grads, preds) of float64 numpy."""
+    params = path_params(model_key, case, dr, dtype)
+    loss, parts = replay.oracle_loss(model_key, case, hp, adj, dr, params, st)
+    loss.backward()
+    out = dict(loss=float(loss), parts={k: float(v) for k, v in parts.items()},
+               grads={k: p.grad.double().numpy() for k, p in params.items()})
+    with torch.no_grad():
+        e = replay.clean_embeds(model_key, adj, hp, params)
+        users, mask = pred_users_mask(case)
+        out['preds'] = O.full_predict(e[:case['n_user']], e[case['n_user']:], users, mask).double().numpy()
+    return out
+
+
+def path_errors(got, ref):
+    """Largest error of each output as a fraction of its bound (<= 1 passes): loss and terms |d| <= 1e-5 max(1, |ref|);
+    gradients 2e-4 |ref| + 5e-6 max|ref|; scores 1e-5 max(1, |ref|)."""
+    def frac(a, b, tol):
+        err = np.abs(np.asarray(a, dtype=np.float64) - b)
+        return float(np.max(np.divide(err, tol, out=np.where(err > 0, np.inf, 0.0), where=tol > 0), initial=0.0))
+    r = {'loss': frac(got['loss'], ref['loss'], LOSS_RTOL * max(1.0, abs(ref['loss'])))}
+    assert set(got['parts']) == set(ref['parts']), (sorted(got['parts']), sorted(ref['parts']))
+    for k, v in ref['parts'].items():
+        r['part_' + k] = frac(got['parts'][k], v, LOSS_RTOL * max(1.0, abs(v)))
+    assert set(got['grads']) == set(ref['grads']), (sorted(got['grads']), sorted(ref['grads']))
+    for k, g in ref['grads'].items():
+        assert got['grads'][k].shape == g.shape, (k, got['grads'][k].shape, g.shape)
+        r['grad_' + k] = frac(got['grads'][k], g, GRAD_RTOL * np.abs(g) + GRAD_MAXTOL * np.abs(g).max())
+    r['preds'] = frac(got['preds'], ref['preds'], PRED_RTOL * np.maximum(1.0, np.abs(ref['preds'])))
+    return r
+
+
+def kink_margin(model_key, case, hp, adj, dr, st):
+    """Smallest |v| / sum|terms of v| over the nonzero float64 values v that a kink of the model acts on (SimGCL's sign(x),
+    HCCF's two LeakyReLUs, LightGCL's clamp at +-5: there the distance to the clamp bound); inf when the model has none.
+    Exact zeros (isolated rows) are exact in float32 too and are skipped."""
+    name = model_key.split('_')[0]
+    best = [np.inf]
+
+    def see(v, terms):
+        v, terms = v.detach().double().numpy(), terms.detach().double().numpy()
+        nz = v != 0
+        if nz.any():
+            best[0] = min(best[0], float((np.abs(v[nz]) / terms[nz]).min()))
+
+    f64 = torch.float64
+    e0 = torch.cat([case['user_e'], case['item_e']], 0).to(f64)
+    if name == 'simgcl':
+        a = adj.torch_coo(f64)
+        for view in dr['uniforms']:
+            x = e0
+            for u in view:
+                pre = O.propagate(a, x)
+                see(pre, O.propagate(a, x.abs()))
+                x = O.perturbed(pre, u, hp['eps'])
+    elif name == 'hccf':
+        nu, keep, slope = case['n_user'], hp['keep_rate'], hp['leaky']
+        x = e0
+        hs = (case['user_e'].to(f64) @ dr['user_w'].to(f64) * hp['mult'], case['item_e'].to(f64) @ dr['item_w'].to(f64) * hp['mult'])
+        for k in range(hp['layer_num']):
+            a = O.edge_dropped(adj, dr['edge_keeps'][k], keep, True, f64)
+            hyp = []
+            for h, kp, xs in zip(hs, dr['hyper_keeps'][k], (x[:nu], x[nu:])):
+                h = h * kp.to(f64) / keep if keep != 1.0 else h
+                inner = h.T @ xs
+                see(inner, h.T.abs() @ xs.abs())
+                act = O.leaky(inner, slope)
+                outer = h @ act
+                see(outer, h.abs() @ act.abs())
+                hyp.append(O.leaky(outer, slope))
+            x = O.propagate(a, x) + torch.cat(hyp, 0)
+    elif name == 'lightgcl':
+        ladj = O.lightgcl_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
+        svd = [torch.from_numpy(st['svd_' + k]).to(f64) for k in ('ut', 'vt', 'u_mul_s', 'v_mul_s')]
+        eu, ei, gu, gi = O.lightgcl_embeds(ladj, case['user_e'].to(f64), case['item_e'].to(f64), hp['layer_num'], *svd)
+        for g, e, idx in ((gu, eu, case['ancs']), (gi, ei, case['poss'])):
+            prod = g[idx] * e[idx] / hp['temp']
+            s = prod.sum(1)
+            see(s.abs() - 5.0, prod.abs().sum(1))
+    return best[0]
+
+
 def close(a, b, rtol, atol, what):
     a = np.asarray(a.detach().cpu() if isinstance(a, torch.Tensor) else a, dtype=np.float64)
     b = np.asarray(b.detach().cpu() if isinstance(b, torch.Tensor) else b, dtype=np.float64)
