@@ -261,6 +261,167 @@ def kink_margin(model_key, case, hp, adj, dr, st):
     return best[0]
 
 
+def golden_loss_grads_close(g, loss, parts, named_params, what=''):
+    """cal_loss and the gradients of a drop-in model against a golden case: loss and terms |d| <= 1e-5 max(1, |ref|);
+    gradients rtol 2e-4 + 5e-6 max|ref| (head, row sums and |.| sum for the large tables the golden stores in part)."""
+    assert abs(loss.item() - float(g['loss'])) <= 1e-5 * max(1.0, abs(float(g['loss']))), (what, loss.item(), float(g['loss']))
+    for k, v in parts.items():
+        assert abs(float(v) - float(g['part_' + k])) <= 1e-5 * max(1.0, abs(float(g['part_' + k]))), (what, k, float(v), float(g['part_' + k]))
+    for name, p in named_params:
+        gr = p.grad
+        if 'grad_' + name in g:
+            ref = g['grad_' + name]
+            close(gr, ref, 2e-4, 5e-6 * np.abs(ref).max() + 1e-9, what + 'grad_' + name)
+        else:
+            ref = g['grad_' + name + '_head']
+            scale = g['grad_' + name + '_abssum'] / gr.numel()
+            close(gr[:32], ref, 2e-4, 2e-4 * scale + 1e-9, what + 'grad_' + name + '_head')
+            close(gr.double().sum(1), g['grad_' + name + '_rowsum'], 1e-3, 1e-3 * scale * gr.shape[1], what + 'grad_' + name + '_rowsum')
+            assert abs(gr.double().abs().sum().item() - g['grad_' + name + '_abssum']) <= 1e-4 * g['grad_' + name + '_abssum'], (what, name)
+
+
+# ---- NCL's k-means, one Lloyd pass (tests/test_gpu_kmeans.py, tests/test_host_kmeans.py) -----------------------------------------
+
+U32 = 2.0 ** -24                      # unit roundoff of fp32
+KMEANS_SMEM_BYTES = 200 * 1024        # ssl_kmeans_workspace's shared-memory budget
+KMEANS_MAX_CTAS = 132                 # one CTA per SM of an H100 SXM
+KMEANS_ROWS_PER_ROUND = 4             # the widest kmeans_assign_kernel<R>, which the workspace is sized for
+KMEANS_EPS = float(np.float32(1e-6))  # the update kernel's empty-cluster guard, as the fp32 constant it is
+
+
+def gamma(m):
+    """gamma_m = m u / (1 - m u): the relative error bound of m chained fp32 roundings."""
+    return m * U32 / (1 - m * U32)
+
+
+def kmeans_smem_floats(K, d, W, R=KMEANS_ROWS_PER_ROUND):
+    """csrc/kmeans_assign.cuh smem_floats: padded centroids, staged rows, W warp slabs and W count rows."""
+    return K * (d + 1) + W * R * d + W * K * d + W * K
+
+
+def kmeans_k_limit(d, W):
+    """The largest K whose launch with W warps fits the shared-memory budget."""
+    R = KMEANS_ROWS_PER_ROUND
+    return (KMEANS_SMEM_BYTES // 4 - W * R * d) // (d + 1 + W * d + W)
+
+
+def kmeans_launch(n, d, K):
+    """ssl_kmeans_workspace's partition restated -> (n_cta, W, rows_per_cta, rows_per_warp), or None when K * d does not fit.
+    W halves from 8 until the launch fits; about 8 rows per warp, at most one CTA per SM."""
+    W = 8
+    while W > 1 and 4 * kmeans_smem_floats(K, d, W) > KMEANS_SMEM_BYTES:
+        W //= 2
+    if 4 * kmeans_smem_floats(K, d, W) > KMEANS_SMEM_BYTES:
+        return None
+    n_cta = min(-(-n // (W * 8)), KMEANS_MAX_CTAS)
+    rows_per_cta = -(-n // n_cta)
+    return n_cta, W, rows_per_cta, -(-rows_per_cta // W)
+
+
+def kmeans_case(n, d, K, seed, device='cpu'):
+    """-> x [n, d], centroids [K, d] (float32) and a given incoming assignment [n] (int64) for one Lloyd pass.
+
+    The centroids are t.rand draws (aug_utils.py:147) with exact ties planted: centroid pairs equal across lanes (k, k + 1),
+    (4, 21) and within one lane (5, 37), (9, 41), and two or three all-zero rows, which is what an empty cluster becomes.
+    Half the rows sit near a centroid drawn uniformly (so duplicates and zeros win rows and their twins stay empty), a
+    quarter are uniform like the centroids (generic near-ties), and the rest are exact copies of a centroid or exact zeros
+    (distance exactly 0)."""
+    g = torch.Generator(device=device).manual_seed(seed)
+    f32 = dict(device=device, dtype=torch.float32)
+    c = torch.rand(K, d, generator=g, **f32)
+    if K >= 3:
+        for z in (K // 3, K - 1, K // 3 + 32):
+            if z < K:
+                c[z] = 0.0
+        for i, j in ((1, 2), (4, 21), (5, 37), (9, 41)):
+            if j < K:
+                c[j] = c[i]
+    src = torch.randint(0, K, (n,), generator=g, device=device)
+    kind = torch.randint(0, 8, (n,), generator=g, device=device)
+    x = c[src] + 0.05 * torch.randn(n, d, generator=g, **f32)
+    x = torch.where((kind >= 4)[:, None], torch.rand(n, d, generator=g, **f32), x)
+    x = torch.where((kind == 6)[:, None], c[src], x)
+    x = torch.where((kind == 7)[:, None], torch.zeros_like(x), x)
+    given = torch.randint(0, K, (n,), generator=g, device=device)
+    return x, c, given
+
+
+def _kmeans_dist64(x, c):
+    """float64 sum_j (x_j - c_j)^2 of every (row, centroid) pair [n, K], in row chunks of about 2^27 elements."""
+    x, c = x.double(), c.double()
+    step = max(1, (1 << 27) // max(1, c.shape[0] * c.shape[1]))
+    return torch.cat([(x[i:i + step, None, :] - c[None]).square().sum(-1) for i in range(0, x.shape[0], step)], 0)
+
+
+def kmeans_pass_check(x, c0, a0, ch0, out, W, n_cta, rows_per_warp):
+    """One Lloyd pass from centroids ``c0`` and incoming assignment ``a0`` (counter value ``ch0``) against float64; ``out``
+    holds the pass's ``assign`` [n], ``cents`` [K, d], ``counts`` [K] and ``changed`` (int).  Asserts, and returns the worst
+    err / bound of the assignment and the centroids:
+
+    - lowest id on exact ties: every row goes to the lowest id of its centroid's class of bit-equal rows;
+    - the assignment: with D the float64 distances, the kernel's fp32 chain (one rounding per difference, d fused
+      multiply-adds) is within gamma_{d+2} D of D.  Where the best and second-best class differ by more than both bounds,
+      the row must go to float64's argmin; elsewhere its distance must be within both bounds of the minimum;
+    - counts == bincount(assign), and changed == ch0 + the number of rows whose assignment differs from a0;
+    - centroids: the float64 mean of each cluster's members, sum / (count + 1e-6).  A member passes through at most
+      rows_per_warp + W + n_cta fp32 additions (its warp's slab, the per-CTA sum over W slabs, the update's sum over n_cta
+      partials) and two more roundings (the denominator, the division): the error is at most gamma_{m+2} sum |x| / (count + 1e-6)
+      over the members.  An empty cluster is exactly 0."""
+    n, d = x.shape
+    K = c0.shape[0]
+    dev = x.device
+    a = out['assign'].to(dev)
+    assert a.dtype == torch.int64 and a.shape == (n,)
+    assert bool(((a >= 0) & (a < K)).all()), 'assignment out of range'
+    cls, inv = torch.unique(c0.to(dev).double(), dim=0, return_inverse=True)
+    lowest = torch.full((cls.shape[0],), K, dtype=torch.int64, device=dev).scatter_reduce(0, inv, torch.arange(K, device=dev), 'amin')
+    canon = lowest[inv]
+    tie_bad = canon[a] != a
+    assert not bool(tie_bad.any()), f'{int(tie_bad.sum())} rows went to a higher id of an exact tie (first: row {int(tie_bad.nonzero()[0])})'
+
+    D = _kmeans_dist64(x, cls)                                                  # [n, classes]
+    bnd = gamma(d + 2) * D
+    got = D.gather(1, inv[a][:, None])[:, 0]
+    best, arg = D.min(1)
+    bb = bnd.gather(1, arg[:, None])[:, 0]
+    if cls.shape[0] > 1:
+        two = D.topk(2, dim=1, largest=False)
+        second, arg2 = two.values[:, 1], two.indices[:, 1]
+        safe = (second - best) > bb + bnd.gather(1, arg2[:, None])[:, 0]
+    else:
+        safe = torch.ones(n, dtype=torch.bool, device=dev)
+    wrong = safe & (a != lowest[arg])
+    assert not bool(wrong.any()), f'{int(wrong.sum())} rows with a clear nearest centroid assigned elsewhere (first: row {int(wrong.nonzero()[0])})'
+    slack = bnd.gather(1, inv[a][:, None])[:, 0] + bb
+    excess = got - best
+    bad = ~(excess <= slack)
+    assert not bool(bad.any()), f'{int(bad.sum())} rows assigned beyond the distance bound, max excess / bound {(excess / slack.clamp_min(1e-300)).max().item():.3e}'
+    r_assign = float((excess / slack.clamp_min(1e-300)).max()) if n else 0.0
+    # the smallest gap between the best and second-best class, as a multiple of both bounds (> 1: the argmin is exact)
+    tie_gap = float(((second - best) / (bb + bnd.gather(1, arg2[:, None])[:, 0]).clamp_min(1e-300)).min()) if cls.shape[0] > 1 else float('inf')
+
+    want = torch.bincount(a, minlength=K)
+    cnt = out['counts'].to(dev).reshape(-1)
+    assert torch.equal(cnt.double(), want.double()), f'counts differ from bincount(assign) in {int((cnt.double() != want.double()).sum())} clusters'
+    ch_want = int(ch0) + int((a != a0.to(dev)).sum())
+    assert int(out['changed']) == ch_want, f'changed {int(out["changed"])}, want {ch_want}'
+
+    x64 = x.double()
+    S = torch.zeros(K, d, dtype=torch.float64, device=dev).index_add_(0, a, x64)
+    A = torch.zeros(K, d, dtype=torch.float64, device=dev).index_add_(0, a, x64.abs())
+    den = want.double()[:, None] + KMEANS_EPS
+    ref = S / den
+    cb = gamma(rows_per_warp + W + n_cta + 2) * A / den
+    c = out['cents'].to(dev).double()
+    empty = want == 0
+    assert torch.equal(c[empty], torch.zeros_like(c[empty])), 'an empty cluster is not exactly 0'
+    err = (c - ref).abs()
+    bad = ~(err <= cb)
+    assert not bool(bad.any()), f'centroids: {int(bad.sum())} / {bad.numel()} off, max err / bound {(err / cb.clamp_min(1e-300)).max().item():.3e}'
+    r_cents = float((err / cb.clamp_min(1e-300)).max())
+    return {'assign': r_assign, 'cents': r_cents, 'tie_gap': tie_gap}
+
+
 def close(a, b, rtol, atol, what):
     a = np.asarray(a.detach().cpu() if isinstance(a, torch.Tensor) else a, dtype=np.float64)
     b = np.asarray(b.detach().cpu() if isinstance(b, torch.Tensor) else b, dtype=np.float64)

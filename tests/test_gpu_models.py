@@ -58,21 +58,8 @@ def test_cal_loss_backward_adam_match_reference(model_key, case_name):
     opt = FusedAdam(model.parameters(), lr=float(g.get('opt_lr', 1e-3)), weight_decay=wd)
     opt.zero_grad()
     loss, parts = model.cal_loss(batch)
-    assert abs(loss.item() - float(g['loss'])) <= 1e-5 * max(1.0, abs(float(g['loss']))), (loss.item(), float(g['loss']))
-    for k, v in parts.items():
-        assert abs(float(v) - float(g['part_' + k])) <= 1e-5 * max(1.0, abs(float(g['part_' + k]))), (k, float(v), float(g['part_' + k]))
     loss.backward()
-    for name, p in model.named_parameters():
-        gr = p.grad
-        if 'grad_' + name in g:
-            ref = g['grad_' + name]
-            H.close(gr, ref, 2e-4, 5e-6 * np.abs(ref).max() + 1e-9, 'grad_' + name)
-        else:
-            ref = g['grad_' + name + '_head']
-            scale = g['grad_' + name + '_abssum'] / gr.numel()
-            H.close(gr[:32], ref, 2e-4, 2e-4 * scale + 1e-9, 'grad_' + name + '_head')
-            H.close(gr.double().sum(1), g['grad_' + name + '_rowsum'], 1e-3, 1e-3 * scale * gr.shape[1], 'grad_' + name + '_rowsum')
-            assert abs(gr.double().abs().sum().item() - g['grad_' + name + '_abssum']) <= 1e-4 * g['grad_' + name + '_abssum']
+    H.golden_loss_grads_close(g, loss, parts, model.named_parameters())
     opt.step()
     for name, p in model.named_parameters():
         full = 'new_' + name in g
