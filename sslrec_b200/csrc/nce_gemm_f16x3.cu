@@ -3,6 +3,7 @@
 //
 //   S  = R C^T   = R_hi C_hi^T + 2^-12 (R_lo C_hi^T + R_hi C_lo^T)
 //   E' = exp2(S - offset) * colscale * 2^14 / M ;  rowsum' += sum_c E'          (M: a power of two >= max |colscale|)
+//   E' = exp2(S - (offset - 14))                       without colscale (M = 1): the bias folded into the offset
 //   O' = E' C    = E'_hi C_hi + 2^-12 (E'_lo C_hi + E'_hi C_lo) ;    O = O' M 2^-14, rowsum = rowsum' M 2^-14
 //
 // Same contract as ssl_softmax_gemm_tf32x3 (nce_gemm_tc.cu) and ssl_softmax_gemm (nce_gemm.cu), at twice the tf32 MMA rate.
@@ -22,6 +23,10 @@
 //   colscale[0, n_c) in the prologue for M, a power of two >= its largest magnitude, and E' carries colscale / M with an
 //   exponent bias of 2^14, so E' <= 2^14 and its hi part is a normal fp16 down to E' = 2^-14.  All of these scalings are
 //   exact, need no host read-back (CUDA-graph capture), and every grid size finds the same M.
+// * The exp phase runs while the other warpgroup's two GEMMs (768 tensor-core clocks at the data-sheet rate) run, and
+//   it took longer than that (profiles/r09_nce_exp_phase.md).  So each launch takes an exp phase specialised for its role
+//   (kExp* flags): the forward folds the 2^14 into the offset and, up to offset 13.5, drops the flush rule, which cannot
+//   fire there (f16x3.cuh); the backward does not sum the row sums nobody reads, and computes O as it always has.
 // Units write disjoint o_part / rowsum_part slices and the order of every sum is fixed: no atomics, bit-identical results
 // from launch to launch and for every grid size.
 #include <cuda.h>
@@ -72,6 +77,23 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
+#ifdef SSL_NCE_PHASES
+// Instrumented build (tools/nce_phases.py only, never part of the library): each consumer warpgroup sums the clock64()
+// cycles it spends in each phase of its tile loop; thread 0 of the warpgroup writes the sums to g_phases[CTA][cw][phase]
+// at the end, read back once by ssl_nce_phases_read.
+enum Phase { kPhFull, kPhBar1, kPhIssue1, kPhWait1, kPhExp, kPhBar2, kPhIssue2, kPhWait2, kPhOther, kPhTiles, kNumPhases };
+constexpr int kPhaseCtas = 256;
+__device__ unsigned long long g_phases[kPhaseCtas * 2 * kNumPhases];
+#define SSL_PHASE(k)                                \
+    do {                                            \
+        const unsigned long long t_ = clock64();    \
+        ph[k] += t_ - ph_t;                         \
+        ph_t = t_;                                  \
+    } while (0)
+#else
+#define SSL_PHASE(k) do { } while (0)
+#endif
+
 __device__ __forceinline__ float ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -156,20 +178,28 @@ __device__ __forceinline__ void wgmma_t(float (&d)[D / 2], const uint32_t *a, ui
     else wgmma_t_n32(d, a, b);
 }
 
+// What the exp phase computes, fixed per launch (launch_f16x3 picks it from the arguments), so that each role issues
+// only the instructions it needs:
+constexpr int kExpColscale = 1;   // colscale != nullptr (the backward): E' = exp2(S - offset) * colscale * 2^14 / M
+                                  // without it (the forward) M = 1 and E' = exp2(S - (offset - 14)): the 2^14 is in the offset
+constexpr int kExpRowsum = 2;     // the row sums are summed (rowsum_part != nullptr, or no colscale)
+constexpr int kExpFlush = 4;      // E' can fall below 2^-14, so hi goes through the flush rule (colscale, or offset > 13.5)
+
 // One 64-column tile: accumulators s / sc (s[4j + 2h + c] = S(row g + 8h, col 8j + 2t + c), g = lane / 4, t = lane % 4)
 // -> E', the two row sums, and E' split into GEMM2's f16 A fragments.  The A fragment of k16 block kk holds
 // a[4kk + 2i + h] = E'(row g + 8h, cols 16kk + 8i + 2t + {0, 1}), i.e. the accumulator pair of column group j = 2kk + i.
-// cscale = 2^14 / M, applied to colscale (or used alone when there is none).
-template <bool CHECK>
+// With colscale, cscale = 2^14 / M scales it and offset is the caller's; without, offset is already offset - 14.
+template <bool CHECK, int EXP>
 __device__ __forceinline__ void exp_tile(const float (&s)[32], const float (&sc)[32], uint32_t (&ahi)[16], uint32_t (&alo)[16],
                                          float offset, const float *__restrict__ cs_ptr, float cscale, int64_t col0, int64_t n_c,
                                          float (&rowsum)[2]) {
+    constexpr bool COLSCALE = EXP & kExpColscale, ROWSUM = EXP & kExpRowsum, FLUSH = EXP & kExpFlush;
     const int t = threadIdx.x & 3;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int64_t col = col0 + 8 * j + 2 * t;
-        float cs0 = cscale, cs1 = cscale;
-        if (cs_ptr != nullptr) {
+        float cs0 = 1.f, cs1 = 1.f;
+        if constexpr (COLSCALE) {
             if (!CHECK) {
                 const float2 c2 = __ldg(reinterpret_cast<const float2 *>(cs_ptr + col));
                 cs0 = c2.x * cscale; cs1 = c2.y * cscale;
@@ -182,22 +212,26 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], const float (&sc)
         for (int h = 0; h < 2; ++h) {
             const float x0 = fmaf(sc[4 * j + 2 * h], ssl::kF16LoUnscale, s[4 * j + 2 * h]);
             const float x1 = fmaf(sc[4 * j + 2 * h + 1], ssl::kF16LoUnscale, s[4 * j + 2 * h + 1]);
-            float e0 = ex2(x0 - offset) * cs0;
-            float e1 = ex2(x1 - offset) * cs1;
+            float e0 = ex2(x0 - offset), e1 = ex2(x1 - offset);
+            if constexpr (COLSCALE) {
+                e0 *= cs0;
+                e1 *= cs1;
+            }
             if (CHECK) {
                 e0 = (col < n_c) ? e0 : 0.f;
                 e1 = (col + 1 < n_c) ? e1 : 0.f;
             }
-            rowsum[h] += e0 + e1;
+            if constexpr (ROWSUM) rowsum[h] += e0 + e1;
             const int q = 4 * (j >> 1) + 2 * (j & 1) + h;
-            ssl::f16x3_split2(e0, e1, ahi[q], alo[q]);
+            ssl::f16x3_split2<FLUSH>(e0, e1, ahi[q], alo[q]);
         }
     }
 }
 
 // LIVE selects a device-side bound (ssl_softmax_gemm_f16x3_live): 0 none (n_live unused), 1 only the first min(*n_live, n_r)
-// rows of R are live, 2 only the first min(*n_live, n_c) rows of C.  n_r stays the row pitch of the outputs.
-template <int D, int LIVE>
+// rows of R are live, 2 only the first min(*n_live, n_c) rows of C.  n_r stays the row pitch of the outputs.  EXP: the
+// kExp* flags of the exp phase; colscale is read if and only if kExpColscale is set.
+template <int D, int LIVE, int EXP>
 __global__ void __launch_bounds__(kNumThreads, 1)
 softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restrict__ R_lo,
                           const __grid_constant__ CUtensorMap map_c_hi, const __grid_constant__ CUtensorMap map_c_lo,
@@ -260,7 +294,7 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
     // M = 2^e >= max |colscale[c]|, c < n_c (frexp: m = f 2^e, f in [0.5, 1)); e is clamped so that 2^(14 - e) and
     // 2^(e - 14) stay normal floats.  Without colscale M = 1.
     int e_m = 0;
-    if (colscale != nullptr) {
+    if constexpr ((EXP & kExpColscale) != 0) {
         float m = 0.f;
         for (int64_t i = threadIdx.x - 128; i < n_c; i += 256) m = fmaxf(m, fabsf(__ldg(colscale + i)));
 #pragma unroll
@@ -273,6 +307,9 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
         e_m = e_m < -100 ? -100 : (e_m > 100 ? 100 : e_m);
     }
     const float cscale = ldexpf(1.f, ssl::kF16Bias - e_m), back = ldexpf(1.f, e_m - ssl::kF16Bias);
+    // without colscale, exp2(S - offset) * 2^14 = exp2(S - (offset - 14)): one subtraction per launch instead of one
+    // multiplication per element
+    const float offset_e = (EXP & kExpColscale) ? offset : offset - (float)ssl::kF16Bias;
 
     float o[D / 2], oc[D / 2], sacc[32], scor[32];
     uint32_t rhi[D / 4], rlo[D / 4], ahi[16], alo[16];
@@ -281,6 +318,9 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
 #pragma unroll
     for (int k = 0; k < 16; ++k) ahi[k] = alo[k] = 0u;
     const uint32_t *rh32 = reinterpret_cast<const uint32_t *>(R_hi), *rl32 = reinterpret_cast<const uint32_t *>(R_lo);
+#ifdef SSL_NCE_PHASES
+    unsigned long long ph[kNumPhases] = {}, ph_t = clock64();
+#endif
     int it = 0;
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
         const int rt = u / n_split, sp = u % n_split;
@@ -306,10 +346,13 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
         float rowsum[2] = {0.f, 0.f};
         for (int tile = t0; tile < t1; ++tile, ++it) {
             const int s = it % ST;
+            SSL_PHASE(kPhOther);
             mbar_wait(&full[s], (it / ST) & 1);
+            SSL_PHASE(kPhFull);
             const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::PART_BYTES;
             // ---- GEMM1: S = R C^T; the two correction products into SC first, then hi*hi into S ----
             named_sync(bar_mine);
+            SSL_PHASE(kPhBar1);
             wg_fence();
 #pragma unroll
             for (int kk = 0; kk < D / 16; ++kk) wgmma_k_n64(scor, rlo + 4 * kk, desc_k<D>(c_hi_a + 32 * kk), kk > 0 ? 1u : 0u);
@@ -319,17 +362,25 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
             for (int kk = 0; kk < D / 16; ++kk) wgmma_k_n64(sacc, rhi + 4 * kk, desc_k<D>(c_hi_a + 32 * kk), kk > 0 ? 1u : 0u);
             wg_commit();
             named_arrive(bar_other);
+            SSL_PHASE(kPhIssue1);
             wg_wait0();
             reg_fence(sacc);
             reg_fence(scor);
             reg_fence(rhi);
             reg_fence(rlo);
+            SSL_PHASE(kPhWait1);
             // ---- E' = exp2(S - offset) * colscale * 2^14 / M, row sums, GEMM2's A fragments ----
             const int64_t col0 = (int64_t)tile * BN;
-            if (col0 + BN <= n_c) exp_tile<false>(sacc, scor, ahi, alo, offset, colscale, cscale, col0, n_c, rowsum);
-            else exp_tile<true>(sacc, scor, ahi, alo, offset, colscale, cscale, col0, n_c, rowsum);
+            if (col0 + BN <= n_c) exp_tile<false, EXP>(sacc, scor, ahi, alo, offset_e, colscale, cscale, col0, n_c, rowsum);
+            else exp_tile<true, EXP>(sacc, scor, ahi, alo, offset_e, colscale, cscale, col0, n_c, rowsum);
             // ---- GEMM2: O' += E' C, the same tiles read MN-major (hi*hi into O, the two correction products into OC) ----
+#ifdef SSL_NCE_PHASES
+            reg_fence(ahi);
+            reg_fence(alo);
+#endif
+            SSL_PHASE(kPhExp);
             named_sync(bar_mine);
+            SSL_PHASE(kPhBar2);
             wg_fence();
 #pragma unroll
             for (int kk = 0; kk < BN / 16; ++kk) wgmma_t<D>(oc, alo + 4 * kk, desc_mn<D>(c_hi_a + kk * 2 * K::GROUP));
@@ -339,20 +390,27 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
             for (int kk = 0; kk < BN / 16; ++kk) wgmma_t<D>(o, ahi + 4 * kk, desc_mn<D>(c_hi_a + kk * 2 * K::GROUP));
             wg_commit();
             named_arrive(bar_other);
+            SSL_PHASE(kPhIssue2);
             // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas
             wg_wait0();
             reg_fence(ahi);
             reg_fence(alo);
             reg_fence(o);
             reg_fence(oc);
+            SSL_PHASE(kPhWait2);
+#ifdef SSL_NCE_PHASES
+            ++ph[kPhTiles];
+#endif
             mbar_arrive(&empty[s]);                               // the tile is consumed by both GEMMs
         }
 
         // ---- unit epilogue: o[4j + 2h + c] = O'(row 16w + g + 8h, col 8j + 2t + c); O = (O + 2^-12 OC) M 2^-14 ----
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
-            rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
+            if constexpr ((EXP & kExpRowsum) != 0) {
+                rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 1);
+                rowsum[h] += __shfl_xor_sync(0xffffffffu, rowsum[h], 2);
+            }
             const int64_t grow = row_a + 8 * h;
             if (grow >= n_r_live) continue;
             float *dst = o_part + ((size_t)sp * n_r + grow) * D;
@@ -361,10 +419,15 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
                 *reinterpret_cast<float2 *>(dst + 8 * j + 2 * t) =
                     make_float2(fmaf(oc[4 * j + 2 * h], ssl::kF16LoUnscale, o[4 * j + 2 * h]) * back,
                                 fmaf(oc[4 * j + 2 * h + 1], ssl::kF16LoUnscale, o[4 * j + 2 * h + 1]) * back);
-            if (t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h] * back;
+            if ((EXP & kExpRowsum) != 0 && t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h] * back;
         }
     }
     if (cw == 0) named_sync(1);                                  // consumer 1's last hand-over
+#ifdef SSL_NCE_PHASES
+    SSL_PHASE(kPhOther);
+    if ((threadIdx.x & 127) == 0 && blockIdx.x < kPhaseCtas)
+        for (int k = 0; k < kNumPhases; ++k) g_phases[(blockIdx.x * 2 + cw) * kNumPhases + k] = ph[k];
+#endif
 }
 
 // ---- host side: tensor maps through the driver entry point (no link-time libcuda dependency) ----
@@ -406,10 +469,10 @@ int make_map(CUtensorMap *map, const uint16_t *base, int64_t rows) {
     return SSL_OK;
 }
 
-template <int D, int LIVE>
-int launch_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo, int64_t n_c,
-                 const float *colscale, float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live,
-                 cudaStream_t st) {
+template <int D, int LIVE, int EXP>
+int launch_f16x3_exp(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo, int64_t n_c,
+                     const float *colscale, float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live,
+                     cudaStream_t st) {
     CUtensorMap mc_hi, mc_lo;
     int rc;
     if ((rc = make_map<D>(&mc_hi, C_hi, n_c)) != SSL_OK) return rc;
@@ -423,7 +486,7 @@ int launch_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const 
     if (dev >= 0 && dev < 64 && configured[dev]) {
         n_sm = sm_count[dev];
     } else {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_f16x3_kernel<D, LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_f16x3_kernel<D, LIVE, EXP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         SSL_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
         if (dev >= 0 && dev < 64) {
             sm_count[dev] = n_sm;
@@ -432,11 +495,25 @@ int launch_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const 
     }
     const int64_t units = ((n_r + BM - 1) / BM) * n_split;
     const int64_t grid = units < n_sm ? units : n_sm;
-    softmax_gemm_f16x3_kernel<D, LIVE><<<(unsigned)grid, kNumThreads, smem, st>>>(
+    softmax_gemm_f16x3_kernel<D, LIVE, EXP><<<(unsigned)grid, kNumThreads, smem, st>>>(
         reinterpret_cast<const __half *>(R_hi), reinterpret_cast<const __half *>(R_lo), mc_hi, mc_lo, n_r, n_c, colscale, offset,
         n_split, rowsum_part, o_part, n_live);
     SSL_LAUNCH_CHECK("softmax_gemm_f16x3_kernel");
     return SSL_OK;
+}
+
+// the exp phase of the launch's role: the backward (colscale, row sums unread), the forward (no colscale; E' >= 2^-13
+// up to offset 13.5, so no flush), or both (colscale and row sums: every flag)
+template <int D, int LIVE>
+int launch_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo, int64_t n_c,
+                 const float *colscale, float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live,
+                 cudaStream_t st) {
+#define SSL_F16X3_LAUNCH(EXP) \
+    launch_f16x3_exp<D, LIVE, EXP>(R_hi, R_lo, n_r, C_hi, C_lo, n_c, colscale, offset, n_split, rowsum_part, o_part, n_live, st)
+    if (colscale != nullptr)
+        return rowsum_part != nullptr ? SSL_F16X3_LAUNCH(kExpColscale | kExpRowsum | kExpFlush) : SSL_F16X3_LAUNCH(kExpColscale | kExpFlush);
+    return offset <= ssl::kF16NoFlushOffset ? SSL_F16X3_LAUNCH(kExpRowsum) : SSL_F16X3_LAUNCH(kExpRowsum | kExpFlush);
+#undef SSL_F16X3_LAUNCH
 }
 
 int check_f16x3_args(const uint16_t *R_hi, const uint16_t *R_lo, const uint16_t *C_hi, const uint16_t *C_lo, int64_t n_c, int32_t dim,
@@ -454,6 +531,17 @@ int check_f16x3_args(const uint16_t *R_hi, const uint16_t *R_lo, const uint16_t 
 }
 
 }  // namespace
+
+#ifdef SSL_NCE_PHASES
+// copies the per-warpgroup phase sums of the last launch (kPhaseCtas x 2 x kNumPhases) to host memory and clears them
+extern "C" int ssl_nce_phases_read(unsigned long long *host, int n) {
+    SSL_CHECK_ARG(n == kPhaseCtas * 2 * kNumPhases, "ssl_nce_phases_read: n must be %d", kPhaseCtas * 2 * kNumPhases);
+    SSL_CUDA(cudaMemcpyFromSymbol(host, g_phases, sizeof(g_phases)));
+    static const unsigned long long zero[kPhaseCtas * 2 * kNumPhases] = {};
+    SSL_CUDA(cudaMemcpyToSymbol(g_phases, zero, sizeof(g_phases)));
+    return SSL_OK;
+}
+#endif
 
 extern "C" int ssl_softmax_gemm_f16x3(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo,
                                       int64_t n_c, int32_t dim, const float *colscale, float offset, int32_t n_split, float *rowsum_part,
