@@ -23,40 +23,11 @@
 // mbarrier complete_tx); the K-major copy of tile t+1 lands while GEMM2 of tile t runs and the
 // row-major copy while GEMM1 of tile t+1 runs, so one buffer each suffices and two CTAs fit
 // per SM at dim <= 64.
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace {
 
 constexpr int BM = 128, BN = 64, EPITCH = BM + 4;
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
 
 // LIVE selects a device-side bound (ssl_softmax_gemm_live): 0 none (n_live unused), 1 only the first min(*n_live, n_r) rows of R
 // are live, 2 only the first min(*n_live, n_c) rows of C.  n_r stays the row pitch of the outputs.
@@ -85,18 +56,18 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
 
     for (int i = tid; i < D * BM + D * BN + BN * D; i += 256) smem[i] = 0.f;
     if (tid == 0) {
-        mbar_init(&bars[0], 1);
-        mbar_init(&bars[1], 1);
+        ssl::mbar_init(&bars[0], 1);
+        ssl::mbar_init(&bars[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     const uint32_t tile_bytes = (uint32_t)(BN * dim * sizeof(float));
     if (tid == 0 && t0 < t1) {
-        mbar_expect_tx(&bars[0], tile_bytes);
-        bulk_g2s(Cs_T, C_t + (size_t)t0 * dim * BN, tile_bytes, &bars[0]);
-        mbar_expect_tx(&bars[1], tile_bytes);
-        bulk_g2s(Cs, C + (size_t)t0 * BN * dim, tile_bytes, &bars[1]);
+        ssl::mbar_expect_tx(&bars[0], tile_bytes);
+        ssl::bulk_g2s(Cs_T, C_t + (size_t)t0 * dim * BN, tile_bytes, &bars[0]);
+        ssl::mbar_expect_tx(&bars[1], tile_bytes);
+        ssl::bulk_g2s(Cs, C + (size_t)t0 * BN * dim, tile_bytes, &bars[1]);
     }
     // resident tile, transposed to K-major (once per CTA)
     {
@@ -131,7 +102,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         for (int i = 0; i < 8; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-        mbar_wait(&bars[0], parity);
+        ssl::mbar_wait(&bars[0], parity);
 #pragma unroll 8
         for (int k = 0; k < dim; ++k) {
             const float4 r0 = *reinterpret_cast<const float4 *>(Rs_T + k * BM + ty * 8);
@@ -146,8 +117,8 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         }
         __syncthreads();   // everyone is done with Cs_T (and with E_T / Cs of the previous tile)
         if (tid == 0 && t + 1 < t1) {
-            mbar_expect_tx(&bars[0], tile_bytes);
-            bulk_g2s(Cs_T, C_t + (size_t)(t + 1) * dim * BN, tile_bytes, &bars[0]);
+            ssl::mbar_expect_tx(&bars[0], tile_bytes);
+            ssl::bulk_g2s(Cs_T, C_t + (size_t)(t + 1) * dim * BN, tile_bytes, &bars[0]);
         }
         // ---------------- exponentials, row sums, transposed store ----------------
 #pragma unroll
@@ -159,7 +130,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
             float e[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-                e[i] = valid ? ex2(s[i][j] - offset) * cs : 0.f;
+                e[i] = valid ? ssl::ex2(s[i][j] - offset) * cs : 0.f;
                 rowsum[i] += e[i];
             }
             *reinterpret_cast<float4 *>(E_T + cl * EPITCH + ty * 8) = make_float4(e[0], e[1], e[2], e[3]);
@@ -167,7 +138,7 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         }
         __syncthreads();   // E_T complete
         // ---------------- GEMM2: O += E . C_tile ----------------
-        mbar_wait(&bars[1], parity);
+        ssl::mbar_wait(&bars[1], parity);
 #pragma unroll 4
         for (int j = 0; j < BN; ++j) {
             const float4 e0 = *reinterpret_cast<const float4 *>(E_T + j * EPITCH + ty * 8);
@@ -192,8 +163,8 @@ softmax_gemm_kernel(const float *__restrict__ R, int64_t n_r, const float *__res
         }
         __syncthreads();   // everyone is done with Cs and E_T
         if (tid == 0 && t + 1 < t1) {
-            mbar_expect_tx(&bars[1], tile_bytes);
-            bulk_g2s(Cs, C + (size_t)(t + 1) * BN * dim, tile_bytes, &bars[1]);
+            ssl::mbar_expect_tx(&bars[1], tile_bytes);
+            ssl::bulk_g2s(Cs, C + (size_t)(t + 1) * BN * dim, tile_bytes, &bars[1]);
         }
     }
 
@@ -220,13 +191,9 @@ template <int D, int LIVE>
 int launch(const float *R, int64_t n_r, const float *C, const float *C_t, int64_t n_c, int dim, const float *colscale,
            float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live, cudaStream_t st) {
     const size_t smem = sizeof(float) * (D * BM + D * BN + BN * D + BN * EPITCH) + 2 * sizeof(uint64_t);
-    static bool configured[64] = {};      // cudaFuncSetAttribute is per device
-    int dev = 0;
-    SSL_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_kernel<D, LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < 64) configured[dev] = true;
-    }
+    int n_sm = 0;
+    const int rc = ssl::configure_once<softmax_gemm_kernel<D, LIVE>>(smem, &n_sm);
+    if (rc != SSL_OK) return rc;
     const int64_t grid = ((n_r + BM - 1) / BM) * n_split;
     softmax_gemm_kernel<D, LIVE><<<(unsigned)grid, 256, smem, st>>>(R, n_r, C, C_t, n_c, dim, colscale, offset, n_split, rowsum_part,
                                                                     o_part, n_live);

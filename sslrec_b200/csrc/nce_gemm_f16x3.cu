@@ -29,11 +29,10 @@
 //   fire there (f16x3.cuh); the backward does not sum the row sums nobody reads, and computes O as it always has.
 // Units write disjoint o_part / rowsum_part slices and the order of every sum is fixed: no atomics, bit-identical results
 // from launch to launch and for every grid size.
-#include <cuda.h>
 #include <cuda_fp16.h>
 #include <cmath>
 
-#include "common.cuh"
+#include "sm90.cuh"
 #include "f16x3.cuh"
 
 namespace {
@@ -51,32 +50,6 @@ template <int D> struct Cfg {
     static constexpr size_t SMEM = 1024 + (size_t)ST * STAGE_BYTES + 2 * ST * sizeof(uint64_t);
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
 #ifdef SSL_NCE_PHASES
 // Instrumented build (tools/nce_phases.py only, never part of the library): each consumer warpgroup sums the clock64()
 // cycles it spends in each phase of its tile loop; thread 0 of the warpgroup writes the sums to g_phases[CTA][cw][phase]
@@ -93,12 +66,6 @@ __device__ unsigned long long g_phases[kPhaseCtas * 2 * kNumPhases];
 #else
 #define SSL_PHASE(k) do { } while (0)
 #endif
-
-__device__ __forceinline__ float ex2(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
 
 // ---- wgmma (sm_90a) ----
 // Shared-memory matrix descriptors over a tile of 64 rows x D fp16, rows ROW_BYTES apart, swizzled by the TMA in repeats
@@ -117,24 +84,6 @@ __device__ __forceinline__ uint64_t desc_mn(uint32_t addr) {
     using K = Cfg<D>;
     return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(K::GROUP >> 4) << 16) | ((uint64_t)(K::GROUP >> 4) << 32) | (K::SWIZZLE << 62);
 }
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// named barriers over the two consumer warpgroups (256 threads); id 0 is __syncthreads'
-__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void named_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
-// keeps registers an asynchronous wgmma reads or writes live (and in place) up to this point
-template <int N>
-__device__ __forceinline__ void reg_fence(float (&r)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
-}
-template <int N>
-__device__ __forceinline__ void reg_fence(uint32_t (&r)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
-}
-
 // GEMM1: d[64 x 64] (+)= A[registers, one k16 block] * B[smem, K-major]^T
 __device__ __forceinline__ void wgmma_k_n64(float (&d)[32], const uint32_t *a, uint64_t b, uint32_t acc) {
     asm volatile(
@@ -212,7 +161,7 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], const float (&sc)
         for (int h = 0; h < 2; ++h) {
             const float x0 = fmaf(sc[4 * j + 2 * h], ssl::kF16LoUnscale, s[4 * j + 2 * h]);
             const float x1 = fmaf(sc[4 * j + 2 * h + 1], ssl::kF16LoUnscale, s[4 * j + 2 * h + 1]);
-            float e0 = ex2(x0 - offset), e1 = ex2(x1 - offset);
+            float e0 = ssl::ex2(x0 - offset), e1 = ssl::ex2(x1 - offset);
             if constexpr (COLSCALE) {
                 e0 *= cs0;
                 e1 *= cs1;
@@ -256,8 +205,8 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_hi));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c_lo));
         for (int s = 0; s < ST; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 256);
+            ssl::mbar_init(&full[s], 1);
+            ssl::mbar_init(&empty[s], 256);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -273,11 +222,11 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
                 const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
                 for (int tile = t0; tile < t1; ++tile, ++it) {
                     const int s = it % ST;
-                    mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
+                    ssl::mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
                     uint8_t *c_hi = ring + s * K::STAGE_BYTES;
-                    mbar_expect_tx(&full[s], K::STAGE_BYTES);
-                    tma_load_2d(c_hi, &map_c_hi, 0, tile * BN, &full[s]);
-                    tma_load_2d(c_hi + K::PART_BYTES, &map_c_lo, 0, tile * BN, &full[s]);
+                    ssl::mbar_expect_tx(&full[s], K::STAGE_BYTES);
+                    ssl::tma_load_2d(c_hi, &map_c_hi, 0, tile * BN, &full[s]);
+                    ssl::tma_load_2d(c_hi + K::PART_BYTES, &map_c_lo, 0, tile * BN, &full[s]);
                 }
             }
         }
@@ -289,7 +238,7 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
     const int cw = wg - 1, w = (threadIdx.x >> 5) & 3, g = lane >> 2, t = lane & 3;
     // ping-pong: named barrier 1 + cw is this warpgroup's turn to issue MMAs (see softmax_gemm_tc_kernel).
     const int bar_mine = 1 + cw, bar_other = 2 - cw;
-    if (cw == 1) named_arrive(1);
+    if (cw == 1) ssl::named_arrive(1);
 
     // M = 2^e >= max |colscale[c]|, c < n_c (frexp: m = f 2^e, f in [0.5, 1)); e is clamped so that 2^(14 - e) and
     // 2^(e - 14) stay normal floats.  Without colscale M = 1.
@@ -300,7 +249,7 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
         if (lane == 0) cs_max[(threadIdx.x - 128) >> 5] = m;
-        named_sync(3);
+        ssl::named_sync(3);
 #pragma unroll
         for (int i = 0; i < 8; ++i) m = fmaxf(m, cs_max[i]);
         frexpf(m, &e_m);
@@ -347,27 +296,27 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
         for (int tile = t0; tile < t1; ++tile, ++it) {
             const int s = it % ST;
             SSL_PHASE(kPhOther);
-            mbar_wait(&full[s], (it / ST) & 1);
+            ssl::mbar_wait(&full[s], (it / ST) & 1);
             SSL_PHASE(kPhFull);
-            const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::PART_BYTES;
+            const uint32_t c_hi_a = ssl::smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::PART_BYTES;
             // ---- GEMM1: S = R C^T; the two correction products into SC first, then hi*hi into S ----
-            named_sync(bar_mine);
+            ssl::named_sync(bar_mine);
             SSL_PHASE(kPhBar1);
-            wg_fence();
+            ssl::wg_fence();
 #pragma unroll
             for (int kk = 0; kk < D / 16; ++kk) wgmma_k_n64(scor, rlo + 4 * kk, desc_k<D>(c_hi_a + 32 * kk), kk > 0 ? 1u : 0u);
 #pragma unroll
             for (int kk = 0; kk < D / 16; ++kk) wgmma_k_n64(scor, rhi + 4 * kk, desc_k<D>(c_lo_a + 32 * kk), 1u);
 #pragma unroll
             for (int kk = 0; kk < D / 16; ++kk) wgmma_k_n64(sacc, rhi + 4 * kk, desc_k<D>(c_hi_a + 32 * kk), kk > 0 ? 1u : 0u);
-            wg_commit();
-            named_arrive(bar_other);
+            ssl::wg_commit();
+            ssl::named_arrive(bar_other);
             SSL_PHASE(kPhIssue1);
-            wg_wait0();
-            reg_fence(sacc);
-            reg_fence(scor);
-            reg_fence(rhi);
-            reg_fence(rlo);
+            ssl::wg_wait0();
+            ssl::reg_fence(sacc);
+            ssl::reg_fence(scor);
+            ssl::reg_fence(rhi);
+            ssl::reg_fence(rlo);
             SSL_PHASE(kPhWait1);
             // ---- E' = exp2(S - offset) * colscale * 2^14 / M, row sums, GEMM2's A fragments ----
             const int64_t col0 = (int64_t)tile * BN;
@@ -375,33 +324,33 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
             else exp_tile<true, EXP>(sacc, scor, ahi, alo, offset_e, colscale, cscale, col0, n_c, rowsum);
             // ---- GEMM2: O' += E' C, the same tiles read MN-major (hi*hi into O, the two correction products into OC) ----
 #ifdef SSL_NCE_PHASES
-            reg_fence(ahi);
-            reg_fence(alo);
+            ssl::reg_fence(ahi);
+            ssl::reg_fence(alo);
 #endif
             SSL_PHASE(kPhExp);
-            named_sync(bar_mine);
+            ssl::named_sync(bar_mine);
             SSL_PHASE(kPhBar2);
-            wg_fence();
+            ssl::wg_fence();
 #pragma unroll
             for (int kk = 0; kk < BN / 16; ++kk) wgmma_t<D>(oc, alo + 4 * kk, desc_mn<D>(c_hi_a + kk * 2 * K::GROUP));
 #pragma unroll
             for (int kk = 0; kk < BN / 16; ++kk) wgmma_t<D>(oc, ahi + 4 * kk, desc_mn<D>(c_lo_a + kk * 2 * K::GROUP));
 #pragma unroll
             for (int kk = 0; kk < BN / 16; ++kk) wgmma_t<D>(o, ahi + 4 * kk, desc_mn<D>(c_hi_a + kk * 2 * K::GROUP));
-            wg_commit();
-            named_arrive(bar_other);
+            ssl::wg_commit();
+            ssl::named_arrive(bar_other);
             SSL_PHASE(kPhIssue2);
             // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas
-            wg_wait0();
-            reg_fence(ahi);
-            reg_fence(alo);
-            reg_fence(o);
-            reg_fence(oc);
+            ssl::wg_wait0();
+            ssl::reg_fence(ahi);
+            ssl::reg_fence(alo);
+            ssl::reg_fence(o);
+            ssl::reg_fence(oc);
             SSL_PHASE(kPhWait2);
 #ifdef SSL_NCE_PHASES
             ++ph[kPhTiles];
 #endif
-            mbar_arrive(&empty[s]);                               // the tile is consumed by both GEMMs
+            ssl::mbar_arrive(&empty[s]);                               // the tile is consumed by both GEMMs
         }
 
         // ---- unit epilogue: o[4j + 2h + c] = O'(row 16w + g + 8h, col 8j + 2t + c); O = (O + 2^-12 OC) M 2^-14 ----
@@ -422,7 +371,7 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
             if ((EXP & kExpRowsum) != 0 && t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h] * back;
         }
     }
-    if (cw == 0) named_sync(1);                                  // consumer 1's last hand-over
+    if (cw == 0) ssl::named_sync(1);                                  // consumer 1's last hand-over
 #ifdef SSL_NCE_PHASES
     SSL_PHASE(kPhOther);
     if ((threadIdx.x & 127) == 0 && blockIdx.x < kPhaseCtas)
@@ -430,71 +379,21 @@ softmax_gemm_f16x3_kernel(const __half *__restrict__ R_hi, const __half *__restr
 #endif
 }
 
-// ---- host side: tensor maps through the driver entry point (no link-time libcuda dependency) ----
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (fn == nullptr) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
-// [rows, D] fp16, row-major -> boxes of D x 64 rows (one row = 128 B with SWIZZLE_128B at D = 64, 64 B with SWIZZLE_64B
-// at D = 32); rows past ``rows`` read as 0
-template <int D>
-int make_map(CUtensorMap *map, const uint16_t *base, int64_t rows) {
-    EncodeTiledFn fn = encode_fn();
-    if (fn == nullptr) {
-        ssl::set_error("cuTensorMapEncodeTiled is not available from this driver");
-        return SSL_E_CUDA;
-    }
-    cuuint64_t gdim[2] = {(cuuint64_t)D, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)D * 2};
-    cuuint32_t box[2] = {(cuuint32_t)D, (cuuint32_t)BN};
-    cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<uint16_t *>(base), gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, D == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        ssl::set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-        return SSL_E_CUDA;
-    }
-    return SSL_OK;
-}
-
 template <int D, int LIVE, int EXP>
 int launch_f16x3_exp(const uint16_t *R_hi, const uint16_t *R_lo, int64_t n_r, const uint16_t *C_hi, const uint16_t *C_lo, int64_t n_c,
                      const float *colscale, float offset, int n_split, float *rowsum_part, float *o_part, const int64_t *n_live,
                      cudaStream_t st) {
+    // [n_c, D] fp16, row-major -> boxes of D x 64 rows (one row = 128 B with SWIZZLE_128B at D = 64, 64 B with SWIZZLE_64B
+    // at D = 32)
+    constexpr CUtensorMapSwizzle SW = D == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     CUtensorMap mc_hi, mc_lo;
     int rc;
-    if ((rc = make_map<D>(&mc_hi, C_hi, n_c)) != SSL_OK) return rc;
-    if ((rc = make_map<D>(&mc_lo, C_lo, n_c)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mc_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, C_hi, n_c, D, D * 2, D, BN, SW)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mc_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, C_lo, n_c, D, D * 2, D, BN, SW)) != SSL_OK) return rc;
     const size_t smem = Cfg<D>::SMEM;
-    // cudaFuncSetAttribute is per DEVICE: remember which devices of this process are configured, and their SM counts
-    static bool configured[64] = {};
-    static int sm_count[64] = {};
-    int dev = 0, n_sm = 0;
-    SSL_CUDA(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && configured[dev]) {
-        n_sm = sm_count[dev];
-    } else {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_f16x3_kernel<D, LIVE, EXP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        SSL_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        if (dev >= 0 && dev < 64) {
-            sm_count[dev] = n_sm;
-            configured[dev] = true;
-        }
-    }
-    const int64_t units = ((n_r + BM - 1) / BM) * n_split;
-    const int64_t grid = units < n_sm ? units : n_sm;
+    int n_sm = 0;
+    if ((rc = ssl::configure_once<softmax_gemm_f16x3_kernel<D, LIVE, EXP>>(smem, &n_sm)) != SSL_OK) return rc;
+    const int64_t grid = ssl::persistent_grid(((n_r + BM - 1) / BM) * n_split, n_sm);
     softmax_gemm_f16x3_kernel<D, LIVE, EXP><<<(unsigned)grid, kNumThreads, smem, st>>>(
         reinterpret_cast<const __half *>(R_hi), reinterpret_cast<const __half *>(R_lo), mc_hi, mc_lo, n_r, n_c, colscale, offset,
         n_split, rowsum_part, o_part, n_live);

@@ -30,10 +30,9 @@
 //   depend on the grid size or on timing.
 //   The two correction products of GEMM2 go to their own accumulator: the tensor core does not round its fp32
 //   accumulations to nearest, so the long hi*hi sum must not also carry them.
-#include <cuda.h>
 #include <cstdlib>
 
-#include "common.cuh"
+#include "sm90.cuh"
 
 namespace {
 
@@ -50,62 +49,12 @@ template <int D> struct Cfg {
     static constexpr size_t SMEM = 1024 + (size_t)ST * STAGE_BYTES + 2 * ST * sizeof(uint64_t);
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
 // ---- wgmma (sm_90a) ----
 // shared-memory matrix descriptor: K-major, SWIZZLE_128B (layout type 1), 8-row core-matrix groups 1024 bytes apart.
 // A K step of 8 tf32 inside the 128-byte swizzle atom advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t wg_desc(uint32_t addr) {
     return (uint64_t)((addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// named barriers over the two consumer warpgroups (256 threads); id 0 is __syncthreads'
-__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void named_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
-// keeps registers an asynchronous wgmma reads or writes live (and in place) up to this point
-template <int N>
-__device__ __forceinline__ void reg_fence(float (&r)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
-}
-template <int N>
-__device__ __forceinline__ void reg_fence(uint32_t (&r)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
-}
-
 // d[64 x 64] (+)= A[registers, one k8 block] * B[smem]^T
 __device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t *a, uint64_t b, uint32_t acc) {
     asm volatile(
@@ -172,8 +121,8 @@ __device__ __forceinline__ void exp_tile(const float (&s)[32], uint32_t (&ahi)[3
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            float e0 = ex2(s[4 * j + 2 * h] - offset) * cs0;
-            float e1 = ex2(s[4 * j + 2 * h + 1] - offset) * cs1;
+            float e0 = ssl::ex2(s[4 * j + 2 * h] - offset) * cs0;
+            float e1 = ssl::ex2(s[4 * j + 2 * h + 1] - offset) * cs1;
             if (CHECK) {
                 e0 = (col < n_c) ? e0 : 0.f;
                 e1 = (col + 1 < n_c) ? e1 : 0.f;
@@ -219,8 +168,8 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ct_hi));
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ct_lo));
         for (int s = 0; s < ST; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 256);
+            ssl::mbar_init(&full[s], 1);
+            ssl::mbar_init(&empty[s], 256);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -237,17 +186,17 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
                 const int t0 = (int)(n_ct * sp / n_split), t1 = (int)(n_ct * (sp + 1) / n_split);
                 for (int tile = t0; tile < t1; ++tile, ++it) {
                     const int s = it % ST;
-                    mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
+                    ssl::mbar_wait(&empty[s], ((it / ST) & 1) ^ 1);
                     uint8_t *c_hi = ring + s * K::STAGE_BYTES, *c_lo = c_hi + K::C_BYTES;
                     uint8_t *ct_hi = c_lo + K::C_BYTES, *ct_lo = ct_hi + K::T_BYTES;
-                    mbar_expect_tx(&full[s], K::STAGE_BYTES);
+                    ssl::mbar_expect_tx(&full[s], K::STAGE_BYTES);
                     for (int c = 0; c < KCH; ++c) {
-                        tma_load_2d(c_hi + c * K::C_CHUNK, &map_c_hi, c * 32, tile * BN, &full[s]);
-                        tma_load_2d(c_lo + c * K::C_CHUNK, &map_c_lo, c * 32, tile * BN, &full[s]);
+                        ssl::tma_load_2d(c_hi + c * K::C_CHUNK, &map_c_hi, c * 32, tile * BN, &full[s]);
+                        ssl::tma_load_2d(c_lo + c * K::C_CHUNK, &map_c_lo, c * 32, tile * BN, &full[s]);
                     }
                     for (int c = 0; c < JCH; ++c) {
-                        tma_load_2d(ct_hi + c * K::T_CHUNK, &map_ct_hi, tile * BN + c * 32, 0, &full[s]);
-                        tma_load_2d(ct_lo + c * K::T_CHUNK, &map_ct_lo, tile * BN + c * 32, 0, &full[s]);
+                        ssl::tma_load_2d(ct_hi + c * K::T_CHUNK, &map_ct_hi, tile * BN + c * 32, 0, &full[s]);
+                        ssl::tma_load_2d(ct_lo + c * K::T_CHUNK, &map_ct_lo, tile * BN + c * 32, 0, &full[s]);
                     }
                 }
             }
@@ -261,7 +210,7 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
     // ping-pong: named barrier 1 + cw is this warpgroup's turn to issue MMAs.  Each warpgroup issues a GEMM, passes the turn
     // and only then waits for it, so one warpgroup's exp phase runs under the other's MMAs.  Consumer 0 goes first.
     const int bar_mine = 1 + cw, bar_other = 2 - cw;
-    if (cw == 1) named_arrive(1);
+    if (cw == 1) ssl::named_arrive(1);
     float o[D / 2], oc[D / 2], sacc[32];
     uint32_t rhi[D / 2], rlo[D / 2], ahi[32], alo[32];
 #pragma unroll
@@ -294,12 +243,12 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
         float rowsum[2] = {0.f, 0.f};
         for (int tile = t0; tile < t1; ++tile, ++it) {
             const int s = it % ST;
-            mbar_wait(&full[s], (it / ST) & 1);
-            const uint32_t c_hi_a = smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::C_BYTES;
+            ssl::mbar_wait(&full[s], (it / ST) & 1);
+            const uint32_t c_hi_a = ssl::smem_u32(ring + s * K::STAGE_BYTES), c_lo_a = c_hi_a + K::C_BYTES;
             const uint32_t t_hi_a = c_lo_a + K::C_BYTES, t_lo_a = t_hi_a + K::T_BYTES;
             // ---- GEMM1: S = R C^T, three tf32 products, the small ones first ----
-            named_sync(bar_mine);
-            wg_fence();
+            ssl::named_sync(bar_mine);
+            ssl::wg_fence();
 #pragma unroll
             for (int part = 0; part < 3; ++part) {
                 const uint32_t *ra = (part == 0) ? rlo : rhi;
@@ -308,19 +257,19 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
                 for (int kk = 0; kk < D / 8; ++kk)
                     wgmma_rs_n64(sacc, ra + 4 * kk, wg_desc(cb + (kk >> 2) * K::C_CHUNK + (kk & 3) * 32), (part > 0 || kk > 0) ? 1u : 0u);
             }
-            wg_commit();
-            named_arrive(bar_other);
-            wg_wait0();
-            reg_fence(sacc);
-            reg_fence(rhi);
-            reg_fence(rlo);
+            ssl::wg_commit();
+            ssl::named_arrive(bar_other);
+            ssl::wg_wait0();
+            ssl::reg_fence(sacc);
+            ssl::reg_fence(rhi);
+            ssl::reg_fence(rlo);
             // ---- E = exp2(S - offset) * colscale, row sums, GEMM2's A fragment ----
             const int64_t col0 = (int64_t)tile * BN;
             if (col0 + BN <= n_c) exp_tile<false>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
             else exp_tile<true>(sacc, ahi, alo, offset, colscale, col0, n_c, rowsum);
             // ---- GEMM2: O += E C (hi*hi into O, the two correction products into OC) ----
-            named_sync(bar_mine);
-            wg_fence();
+            ssl::named_sync(bar_mine);
+            ssl::wg_fence();
 #pragma unroll
             for (int part = 0; part < 3; ++part) {
                 const uint32_t *ea = (part == 0) ? alo : ahi;
@@ -332,15 +281,15 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
                     else wgmma_rs<D>(oc, ea + 4 * kk, bd);
                 }
             }
-            wg_commit();
-            named_arrive(bar_other);
+            ssl::wg_commit();
+            ssl::named_arrive(bar_other);
             // waiting here rather than under the next GEMM1 keeps ptxas from serialising the wgmmas
-            wg_wait0();
-            reg_fence(ahi);
-            reg_fence(alo);
-            reg_fence(o);
-            reg_fence(oc);
-            mbar_arrive(&empty[s]);                               // both copies of the tile are consumed
+            ssl::wg_wait0();
+            ssl::reg_fence(ahi);
+            ssl::reg_fence(alo);
+            ssl::reg_fence(o);
+            ssl::reg_fence(oc);
+            ssl::mbar_arrive(&empty[s]);                               // both copies of the tile are consumed
         }
 
         // ---- unit epilogue: o[4j + 2h + c] = O(row 16w + g + 8h, col 8j + 2t + c) ----
@@ -358,79 +307,30 @@ softmax_gemm_tc_kernel(const float *__restrict__ R_hi, const float *__restrict__
             if (t == 0 && rowsum_part != nullptr) rowsum_part[(size_t)sp * n_r + grow] = rowsum[h];
         }
     }
-    if (cw == 0) named_sync(1);                                  // consumer 1's last hand-over
-}
-
-// ---- host side: tensor maps through the driver entry point (no link-time libcuda dependency) ----
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (fn == nullptr) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
-// [rows, cols] fp32, row pitch ``pitch`` floats -> boxes of 32 floats (128 B, SWIZZLE_128B) x box_rows rows;
-// out-of-range rows / columns read as 0
-int make_map(CUtensorMap *map, const float *base, int64_t rows, int64_t cols, int64_t pitch, int box_rows) {
-    EncodeTiledFn fn = encode_fn();
-    if (fn == nullptr) {
-        ssl::set_error("cuTensorMapEncodeTiled is not available from this driver");
-        return SSL_E_CUDA;
-    }
-    cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)pitch * sizeof(float)};
-    cuuint32_t box[2] = {32u, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        ssl::set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-        return SSL_E_CUDA;
-    }
-    return SSL_OK;
+    if (cw == 0) ssl::named_sync(1);                                  // consumer 1's last hand-over
 }
 
 template <int D, int LIVE>
 int launch_tc(const float *R_hi, const float *R_lo, int64_t n_r, const float *C_hi, const float *C_lo, const float *CT_hi,
               const float *CT_lo, int64_t ct_pitch, int64_t n_c, const float *colscale, float offset, int n_split,
               float *rowsum_part, float *o_part, const int64_t *n_live, cudaStream_t st) {
+    // fp32 boxes of 32 floats (128 B, SWIZZLE_128B) x 64 rows of C, x D rows of C^T [D, ct_pitch]
+    constexpr CUtensorMapDataType F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    constexpr CUtensorMapSwizzle SW = CU_TENSOR_MAP_SWIZZLE_128B;
     CUtensorMap mc_hi, mc_lo, mt_hi, mt_lo;
     int rc;
-    if ((rc = make_map(&mc_hi, C_hi, n_c, D, D, BN)) != SSL_OK) return rc;
-    if ((rc = make_map(&mc_lo, C_lo, n_c, D, D, BN)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mc_hi, F32, C_hi, n_c, D, D * 4, 32, BN, SW)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mc_lo, F32, C_lo, n_c, D, D * 4, 32, BN, SW)) != SSL_OK) return rc;
     // the transposed copy's columns are permuted within groups of 8 (see exp_tile): its last group is read whole
     const int64_t n_c8 = (n_c + 7) / 8 * 8;
-    if ((rc = make_map(&mt_hi, CT_hi, D, n_c8, ct_pitch, D)) != SSL_OK) return rc;
-    if ((rc = make_map(&mt_lo, CT_lo, D, n_c8, ct_pitch, D)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mt_hi, F32, CT_hi, D, n_c8, ct_pitch * 4, 32, D, SW)) != SSL_OK) return rc;
+    if ((rc = ssl::make_map_2d(&mt_lo, F32, CT_lo, D, n_c8, ct_pitch * 4, 32, D, SW)) != SSL_OK) return rc;
     const size_t smem = Cfg<D>::SMEM;
-    // cudaFuncSetAttribute is per DEVICE: remember which devices of this process are configured, and their SM counts
-    static bool configured[64] = {};
-    static int sm_count[64] = {};
-    int dev = 0, n_sm = 0;
-    SSL_CUDA(cudaGetDevice(&dev));
-    if (dev >= 0 && dev < 64 && configured[dev]) {
-        n_sm = sm_count[dev];
-    } else {
-        SSL_CUDA(cudaFuncSetAttribute(softmax_gemm_tc_kernel<D, LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        SSL_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        if (dev >= 0 && dev < 64) {
-            sm_count[dev] = n_sm;
-            configured[dev] = true;
-        }
-    }
-    // persistent: one CTA per SM, each looping over units (R tile, C chunk) blockIdx.x, + gridDim.x, ...; sized for the
-    // capacity when the live count is on the device (the units past it are skipped, the live ones stay spread round-robin)
-    const int64_t units = ((n_r + BM - 1) / BM) * n_split;
-    const int64_t grid = units < n_sm ? units : n_sm;
+    int n_sm = 0;
+    if ((rc = ssl::configure_once<softmax_gemm_tc_kernel<D, LIVE>>(smem, &n_sm)) != SSL_OK) return rc;
+    // units (R tile, C chunk), sized for the capacity when the live count is on the device (the units past it are skipped,
+    // the live ones stay spread round-robin)
+    const int64_t grid = ssl::persistent_grid(((n_r + BM - 1) / BM) * n_split, n_sm);
     softmax_gemm_tc_kernel<D, LIVE><<<(unsigned)grid, kNumThreads, smem, st>>>(R_hi, R_lo, mc_hi, mc_lo, mt_hi, mt_lo, n_r, n_c, colscale,
                                                                                offset, n_split, rowsum_part, o_part, n_live);
     SSL_LAUNCH_CHECK("softmax_gemm_tc_kernel");

@@ -15,6 +15,7 @@ gradient is ever materialised per loss term or added by torch.
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
@@ -759,6 +760,9 @@ def bpr_loss_sum(users: Rows, items: Rows, ancs, poss, negs) -> torch.Tensor:
     return _BprFn.apply(users, items, ancs, poss, negs, *_tokens(users, items))
 
 
+# cached: every eager step asks again for the same few shapes, and the search over splits costs up to tens of
+# microseconds of host time per call, on a step whose rate follows the host's enqueue on some hosts (r09 §7)
+@functools.lru_cache(maxsize=1024)
 def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_few: bool = False) -> int:
     """Number of chunks the streamed operand is cut into: n_rtiles * n_split CTAs on ``slots`` resident-CTA slots (2 per SM for
     the FFMA kernel at dim <= 64, 1 per SM for the tensor-core kernel), every CTA keeping >= 4 tiles.
@@ -785,103 +789,131 @@ def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_f
     return max(effs, key=lambda t: (round(t[0], 9), -t[1]))[1]
 
 
+def contraction_kind(d: int, offset: float, raw: bool = False) -> str:
+    """The InfoNCE contraction kernel for rows of width ``d`` at ``offset``: 'ffma' (FP32 FMA, any d), 'tf32x3' (3xTF32 on the
+    tensor cores: raw rows, which the 3xFP16 operand bound does not cover, and offsets above F16X3_MAX_OFFSET) or 'f16x3'."""
+    if not USE_TENSOR_CORES or d not in (32, 64):
+        return 'ffma'
+    if raw or not f16x3_applies(offset):
+        return 'tf32x3'
+    return 'f16x3'
+
+
+@dataclass
+class Operand:
+    """One side of the contraction: ``n`` rows, ``hat`` [npad, d] (normalised, scaled, zero-padded) and ``rinv`` [max(n, 1)]
+    (None for raw rows), plus the copies the ``kind`` kernel reads (None: hat and rinv only): the FFMA kernel's K-major tile
+    copy ``t`` [npad / 64, d, 64], the tensor-core kernels' hi / lo split [npad, d] (fp16 for 3xFP16) and 3xTF32's
+    transposed split ``thi`` / ``tlo`` [d, npad]."""
+    kind: Optional[str]
+    n: int
+    npad: int
+    hat: torch.Tensor
+    rinv: Optional[torch.Tensor]
+    t: Optional[torch.Tensor] = None
+    hi: Optional[torch.Tensor] = None
+    lo: Optional[torch.Tensor] = None
+    thi: Optional[torch.Tensor] = None
+    tlo: Optional[torch.Tensor] = None
+
+
+def _operand(rows: Rows, idx, norm_mode: int, alpha: float, s: int, kind: Optional[str] = None, streamed: bool = False,
+             npad: Optional[int] = None) -> Operand:
+    """rows[idx] (every row when ``idx`` is None) normalised by ``norm_mode`` (3: raw rows) and scaled by ``alpha``, with the
+    copies the ``kind`` kernel reads of its resident operand R or, ``streamed``, also of its streamed operand C (3xFP16 reads
+    its hi / lo parts in both roles).  ``npad`` defaults to ceil64(n)."""
+    n, d, dev = (rows.n if idx is None else idx.numel()), rows.dim, rows.base.device
+    npad = ceil_to(n, 64) if npad is None else npad
+    f = dict(device=dev, dtype=torch.float32)
+    op = Operand(kind, n, npad, torch.empty(npad, d, **f), None if norm_mode == 3 else torch.empty(max(n, 1), **f))
+    if kind == 'f16x3':
+        op.hi, op.lo = torch.empty(npad, d, device=dev, dtype=torch.float16), torch.empty(npad, d, device=dev, dtype=torch.float16)
+        check(lib.ssl_rows_normalize_f16x3(rows.ptr, rows.stride, _ptr(idx), n, d, norm_mode, alpha, op.hat.data_ptr(),
+                                           op.rinv.data_ptr(), op.hi.data_ptr(), op.lo.data_ptr(), s), 'ssl_rows_normalize_f16x3')
+        return op
+    if kind == 'tf32x3':
+        op.hi, op.lo = torch.empty(npad, d, **f), torch.empty(npad, d, **f)
+        if streamed:
+            op.thi, op.tlo = torch.empty(d, npad, **f), torch.empty(d, npad, **f)
+    elif kind == 'ffma' and streamed:
+        op.t = torch.empty(npad // 64, d, 64, **f)
+    check(lib.ssl_rows_normalize(rows.ptr, rows.stride, _ptr(idx), n, d, norm_mode, alpha, op.hat.data_ptr(), _ptr(op.t),
+                                 _ptr(op.rinv), _ptr(op.hi), _ptr(op.lo), _ptr(op.thi), _ptr(op.tlo), 0 if kind is None else npad, s),
+          'ssl_rows_normalize')
+    return op
+
+
+def _n_split(R: Operand, C: Operand) -> int:
+    """choose_split for a contraction of R against C on their kernel: the tensor-core kernels are persistent, one CTA per SM."""
+    tc = R.kind != 'ffma'
+    return choose_split((R.n + 127) // 128, C.npad // 64, slots=NUM_SM if tc else 2 * NUM_SM, prefer_few=tc)
+
+
+_GEMM_ENTRY = dict(ffma='ssl_softmax_gemm', tf32x3='ssl_softmax_gemm_tf32x3', f16x3='ssl_softmax_gemm_f16x3')
+
+
+def _contract(R: Operand, C: Operand, colscale, offset: float, n_split: int, rowsum_part, o_part, s: int, live=None,
+              live_role: int = LIVE_ROWS):
+    """One launch of the contraction of R against C on their kernel, timed as the forward role (R = anchors) or, with
+    ``colscale``, the backward role (R = table, C = anchors).  ``live``: the device count that bounds the ``live_role`` side."""
+    name = _GEMM_ENTRY[R.kind] + ('' if live is None else '_live')
+    if R.kind == 'ffma':
+        ops = (R.hat.data_ptr(), R.n, C.hat.data_ptr(), C.t.data_ptr(), C.n)
+    elif R.kind == 'tf32x3':
+        ops = (R.hi.data_ptr(), R.lo.data_ptr(), R.n, C.hi.data_ptr(), C.lo.data_ptr(), C.thi.data_ptr(), C.tlo.data_ptr(), C.npad, C.n)
+    else:
+        ops = (R.hi.data_ptr(), R.lo.data_ptr(), R.n, C.hi.data_ptr(), C.lo.data_ptr(), C.n)
+    tail = () if live is None else (live.data_ptr(), live_role)
+    d, bwd = R.hat.shape[1], colscale is not None
+    meta = dict(B=C.n, n=R.n) if bwd else dict(B=R.n, n=C.n)
+    with _timed('nce_gemm_bwd' if bwd else 'nce_gemm_fwd', dict(meta, dim=d, tc=R.kind != 'ffma')):
+        check(getattr(lib, name)(*ops, d, _ptr(colscale), offset, n_split, _ptr(rowsum_part), o_part.data_ptr(), *tail, s),
+              f'{name}({"bwd" if bwd else "fwd"})')
+
+
 def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, deno_eps, live=None):
     """``live``: optional int64 DEVICE scalar; only the first ``*live`` of the ``idx`` rows are anchors (a padded list of
     capacity idx.numel(), see ``dense_infonce_spec_nodes_mean_dev``).  Shapes and n_split then depend on the capacity only."""
     dev = table.base.device
     table.require_whole('an InfoNCE table operand')
-    d = table.dim
-    B, n = idx.numel(), table.n
-    Bp, npad = ceil_to(B, 64), ceil_to(n, 64)
+    d, B = table.dim, idx.numel()
     f = dict(device=dev, dtype=torch.float32)
-    a_hat, rinv1 = torch.empty(Bp, d, **f), torch.empty(B, **f)
-    a_t = torch.empty(Bp // 64, d, 64, **f)
-    p_hat, rinv2 = torch.empty(Bp, d, **f), torch.empty(B, **f)
     comm = table.comm
-    full_table = table
+    full_table, npad = table, None
     if live is not None and (comm is not None or not mean):
         raise RuntimeError('a device-bounded InfoNCE term is a mean on one GPU')
     if comm is not None:                  # contract only this rank's rows of the table; partials are all-reduced
         lo, hi = comm.side_range(table.off, table.n)
         table = table.sub(lo, hi)
-        n = table.n
-        npad = max(64, ceil_to(n, 64))
+        npad = max(64, ceil_to(table.n, 64))
     off = LOG2E / tau
-    use_tc = USE_TENSOR_CORES and d in (32, 64)     # tensor-core contraction; other dims run the FFMA kernel
-    f16 = use_tc and f16x3_applies(off)              # 3xFP16 where its operand bound holds, else 3xTF32
-    t_hat, rinv_t = torch.empty(npad, d, **f), torch.empty(max(n, 1), **f)
-    a_hi = a_lo = t_hi = t_lo = a_thi = a_tlo = t_thi = t_tlo = t_t = None
-    if f16:
-        a_t = None
-        h = dict(device=dev, dtype=torch.float16)
-        a_hi, a_lo, t_hi, t_lo = torch.empty(Bp, d, **h), torch.empty(Bp, d, **h), torch.empty(npad, d, **h), torch.empty(npad, d, **h)
-    elif use_tc:
-        a_t = None
-        a_hi, a_lo, a_thi, a_tlo = torch.empty(Bp, d, **f), torch.empty(Bp, d, **f), torch.empty(d, Bp, **f), torch.empty(d, Bp, **f)
-        t_hi, t_lo, t_thi, t_tlo = torch.empty(npad, d, **f), torch.empty(npad, d, **f), torch.empty(d, npad, **f), torch.empty(d, npad, **f)
-    else:
-        t_t = torch.empty(npad // 64, d, 64, **f)
-    n_split = choose_split((B + 127) // 128, npad // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
-    rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
+    kind = contraction_kind(d, off)
     rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
     with torch.cuda.device(dev):
         s = _stream(table.base)
-        if f16:
-            check(lib.ssl_rows_normalize_f16x3(e1.ptr, e1.stride, idx.data_ptr(), B, d, norm_mode, off, a_hat.data_ptr(),
-                                               rinv1.data_ptr(), a_hi.data_ptr(), a_lo.data_ptr(), s), 'ssl_rows_normalize_f16x3(e1)')
-        else:
-            check(lib.ssl_rows_normalize(e1.ptr, e1.stride, idx.data_ptr(), B, d, norm_mode, off, a_hat.data_ptr(),
-                                         _ptr(a_t), rinv1.data_ptr(), _ptr(a_hi), _ptr(a_lo), _ptr(a_thi), _ptr(a_tlo), Bp, s),
-                  'ssl_rows_normalize(e1)')
-        check(lib.ssl_rows_normalize(e2.ptr, e2.stride, idx2.data_ptr(), B, d, norm_mode, 1.0, p_hat.data_ptr(), None,
-                                     rinv2.data_ptr(), None, None, None, None, 0, s), 'ssl_rows_normalize(e2)')
-        if f16:
-            check(lib.ssl_rows_normalize_f16x3(table.ptr, table.stride, None, n, d, norm_mode, 1.0, t_hat.data_ptr(),
-                                               rinv_t.data_ptr(), t_hi.data_ptr(), t_lo.data_ptr(), s), 'ssl_rows_normalize_f16x3(table)')
-        else:
-            check(lib.ssl_rows_normalize(table.ptr, table.stride, None, n, d, norm_mode, 1.0, t_hat.data_ptr(),
-                                         _ptr(t_t), rinv_t.data_ptr(), _ptr(t_hi), _ptr(t_lo), _ptr(t_thi), _ptr(t_tlo), npad, s),
-                  'ssl_rows_normalize(table)')
-        with _timed('nce_gemm_fwd', dict(B=B, n=n, dim=d, tc=use_tc)):
-            if f16 and live is not None:
-                check(lib.ssl_softmax_gemm_f16x3_live(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), n, d, None, off,
-                                                      n_split, rs_part.data_ptr(), o_part.data_ptr(), live.data_ptr(), LIVE_ROWS, s),
-                      'ssl_softmax_gemm_f16x3_live(fwd)')
-            elif f16:
-                check(lib.ssl_softmax_gemm_f16x3(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), n, d, None, off,
-                                                 n_split, rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm_f16x3(fwd)')
-            elif use_tc and live is not None:
-                check(lib.ssl_softmax_gemm_tf32x3_live(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), t_thi.data_ptr(),
-                                                       t_tlo.data_ptr(), npad, n, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(),
-                                                       live.data_ptr(), LIVE_ROWS, s), 'ssl_softmax_gemm_tf32x3_live(fwd)')
-            elif use_tc:
-                check(lib.ssl_softmax_gemm_tf32x3(a_hi.data_ptr(), a_lo.data_ptr(), B, t_hi.data_ptr(), t_lo.data_ptr(), t_thi.data_ptr(),
-                                                  t_tlo.data_ptr(), npad, n, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(), s),
-                      'ssl_softmax_gemm_tf32x3(fwd)')
-            elif live is not None:
-                check(lib.ssl_softmax_gemm_live(a_hat.data_ptr(), B, t_hat.data_ptr(), t_t.data_ptr(), n, d, None, off, n_split,
-                                                rs_part.data_ptr(), o_part.data_ptr(), live.data_ptr(), LIVE_ROWS, s), 'ssl_softmax_gemm_live(fwd)')
-            else:
-                check(lib.ssl_softmax_gemm(a_hat.data_ptr(), B, t_hat.data_ptr(), t_t.data_ptr(), n, d, None, off, n_split,
-                                           rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm(fwd)')
+        # anchors and table are R and C here and C and R in the backward: both get the copies of either role
+        a = _operand(e1, idx, norm_mode, off, s, kind, streamed=True)
+        p = _operand(e2, idx2, norm_mode, 1.0, s)
+        t = _operand(table, None, norm_mode, 1.0, s, kind, streamed=True, npad=npad)
+        n_split = _n_split(a, t)
+        rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
+        _contract(a, t, None, off, n_split, rs_part, o_part, s, live, LIVE_ROWS)
         if comm is not None:
             red = torch.cat([o_part.sum(0), rs_part.sum(0).unsqueeze(1)], 1)         # [B, d+1]
             comm.allreduce_sum(red)
             o_part, rs_part, n_split = red[:, :d].contiguous().unsqueeze(0), red[:, d].contiguous().unsqueeze(0), 1
-        check(lib.ssl_nce_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, a_hat.data_ptr(), p_hat.data_ptr(),
+        check(lib.ssl_nce_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, a.hat.data_ptr(), p.hat.data_ptr(),
                                    tau, deno_eps * math.exp(-1.0 / tau), rowsum.data_ptr(), obar.data_ptr(),
                                    loss_b.data_ptr(), s), 'ssl_nce_finalize')
         if live is not None:          # (1 / live) sum_{b < live} loss_b: the padding rows' values are never read
             check(lib.ssl_sum_live(loss_b.data_ptr(), B, live.data_ptr(), 1.0, out.data_ptr(), s), 'ssl_sum_live')
         else:
             check(lib.ssl_sum(loss_b.data_ptr(), B, (1.0 / B) if mean else 1.0, out.data_ptr(), s), 'ssl_sum')
-    saved = (e1, e2, table, idx, tau, mean, a_hat, a_t, p_hat, rinv1, rinv2, t_hat, rinv_t, rowsum, obar, full_table, comm,
-             (a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo) if use_tc else None, live)
-    return out, saved
+    return out, (e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live)
 
 
 def _nce_bwd(saved, g):
-    (e1, e2, table, idx, tau, mean, a_hat, a_t, p_hat, rinv1, rinv2, t_hat, rinv_t, rowsum, obar, full_table, comm, tc, live) = saved
+    e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live = saved
     dev, d = g.device, table.dim
     B, n = idx.numel(), table.n
     g = g.contiguous()
@@ -896,53 +928,24 @@ def _nce_bwd(saved, g):
             local_dt = torch.zeros(comm.side_block(full_table.n), d, **f)
             gt, gt_stride = local_dt.data_ptr(), d
         if live is not None and (g1 is not None or g2 is not None):        # rows b < live only, mean over live
-            check(lib.ssl_nce_bwd_rows_live(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
+            check(lib.ssl_nce_bwd_rows_live(a.hat.data_ptr(), p.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), p.rinv.data_ptr(),
                                             idx.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, g1, e1.grad_stride, g2, e2.grad_stride, s),
                   'ssl_nce_bwd_rows_live')
         elif g1 is not None or g2 is not None:
-            check(lib.ssl_nce_bwd_rows(a_hat.data_ptr(), p_hat.data_ptr(), obar.data_ptr(), rinv1.data_ptr(), rinv2.data_ptr(),
+            check(lib.ssl_nce_bwd_rows(a.hat.data_ptr(), p.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), p.rinv.data_ptr(),
                                        idx.data_ptr(), B, d, tau, g.data_ptr(), scale, g1, e1.grad_stride, g2, e2.grad_stride, s),
                   'ssl_nce_bwd_rows')
         if gt is not None and n > 0:
-            colscale = torch.zeros(ceil_to(B, 64), **f)   # padded tail is read (then masked) by the tile loads
+            colscale = torch.zeros(a.npad, **f)   # padded tail is read (then masked) by the tile loads
             if live is not None:          # 0 past the live anchors
                 check(lib.ssl_nce_colscale_live(rowsum.data_ptr(), B, live.data_ptr(), g.data_ptr(), 1.0, colscale.data_ptr(), s),
                       'ssl_nce_colscale_live')
             else:
                 check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), scale, colscale.data_ptr(), s), 'ssl_nce_colscale')
-            f16 = bool(tc) and tc[0].dtype == torch.float16
-            n_split = choose_split((n + 127) // 128, ceil_to(B, 64) // 64, slots=NUM_SM if tc else 2 * NUM_SM, prefer_few=bool(tc))
+            n_split = _n_split(t, a)
             dt_part = torch.empty(n_split, n, d, **f)
-            with _timed('nce_gemm_bwd', dict(B=B, n=n, dim=d, tc=bool(tc))):
-                if f16 and live is not None:
-                    a_hi, a_lo, _, _, t_hi, t_lo = tc
-                    check(lib.ssl_softmax_gemm_f16x3_live(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), B, d,
-                                                          colscale.data_ptr(), LOG2E / tau, n_split, None, dt_part.data_ptr(),
-                                                          live.data_ptr(), LIVE_COLS, s), 'ssl_softmax_gemm_f16x3_live(bwd)')
-                elif f16:
-                    a_hi, a_lo, _, _, t_hi, t_lo = tc
-                    check(lib.ssl_softmax_gemm_f16x3(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), B, d,
-                                                     colscale.data_ptr(), LOG2E / tau, n_split, None, dt_part.data_ptr(), s),
-                          'ssl_softmax_gemm_f16x3(bwd)')
-                elif tc and live is not None:
-                    a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo = tc
-                    check(lib.ssl_softmax_gemm_tf32x3_live(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), a_thi.data_ptr(),
-                                                           a_tlo.data_ptr(), a_thi.shape[1], B, d, colscale.data_ptr(), LOG2E / tau, n_split, None,
-                                                           dt_part.data_ptr(), live.data_ptr(), LIVE_COLS, s), 'ssl_softmax_gemm_tf32x3_live(bwd)')
-                elif live is not None:
-                    check(lib.ssl_softmax_gemm_live(t_hat.data_ptr(), n, a_hat.data_ptr(), a_t.data_ptr(), B, d, colscale.data_ptr(),
-                                                    LOG2E / tau, n_split, None, dt_part.data_ptr(), live.data_ptr(), LIVE_COLS, s),
-                          'ssl_softmax_gemm_live(bwd)')
-                elif tc:
-                    a_hi, a_lo, a_thi, a_tlo, t_hi, t_lo = tc
-                    Bp = a_thi.shape[1]
-                    check(lib.ssl_softmax_gemm_tf32x3(t_hi.data_ptr(), t_lo.data_ptr(), n, a_hi.data_ptr(), a_lo.data_ptr(), a_thi.data_ptr(),
-                                                      a_tlo.data_ptr(), Bp, B, d, colscale.data_ptr(), LOG2E / tau, n_split, None,
-                                                      dt_part.data_ptr(), s), 'ssl_softmax_gemm_tf32x3(bwd)')
-                else:
-                    check(lib.ssl_softmax_gemm(t_hat.data_ptr(), n, a_hat.data_ptr(), a_t.data_ptr(), B, d, colscale.data_ptr(),
-                                               LOG2E / tau, n_split, None, dt_part.data_ptr(), s), 'ssl_softmax_gemm(bwd)')
-            check(lib.ssl_nce_bwd_table(dt_part.data_ptr(), n_split, t_hat.data_ptr(), rinv_t.data_ptr(), n, d, gt,
+            _contract(t, a, colscale, LOG2E / tau, n_split, None, dt_part, s, live, LIVE_COLS)
+            check(lib.ssl_nce_bwd_table(dt_part.data_ptr(), n_split, t.hat.data_ptr(), t.rinv.data_ptr(), n, d, gt,
                                         gt_stride, 1, s), 'ssl_nce_bwd_table')
         if local_dt is not None:
             dense = comm.allgather_side(local_dt, full_table.n)
@@ -976,33 +979,6 @@ def infonce_loss_sum(e1: Rows, e2: Rows, table: Rows, idx, temp: float, idx2=Non
 
 # ---- LightGCL: log-sum-exp of raw (un-normalised) rows against a raw table (lightgcl.py:112-113) -------------
 
-def _raw_operand(x: torch.Tensor, alpha: float, use_tc: bool):
-    """x * alpha with the copies the contraction reads in either role (resident R or streamed C): norm_mode 3."""
-    n, d = x.shape
-    npad = max(64, ceil_to(n, 64))
-    f = dict(device=x.device, dtype=torch.float32)
-    out = torch.empty(npad, d, **f)
-    hi = lo = thi = tlo = out_t = None
-    if use_tc:
-        hi, lo, thi, tlo = torch.empty(npad, d, **f), torch.empty(npad, d, **f), torch.empty(d, npad, **f), torch.empty(d, npad, **f)
-    else:
-        out_t = torch.empty(npad // 64, d, 64, **f)
-    with torch.cuda.device(x.device):
-        check(lib.ssl_rows_normalize(x.data_ptr(), x.stride(0), None, n, d, 3, alpha, out.data_ptr(), _ptr(out_t), None,
-                                     _ptr(hi), _ptr(lo), _ptr(thi), _ptr(tlo), npad, _stream(x)), 'ssl_rows_normalize(raw)')
-    return out, out_t, hi, lo, thi, tlo, npad
-
-
-def _gemm(use_tc, R, n_r, C, n_c, d, colscale, offset, n_split, rs_part, o_part, s, what):
-    """One launch of the contraction in either implementation; R / C are ``_raw_operand`` tuples."""
-    if use_tc:
-        check(lib.ssl_softmax_gemm_tf32x3(R[2].data_ptr(), R[3].data_ptr(), n_r, C[2].data_ptr(), C[3].data_ptr(), C[4].data_ptr(),
-                                          C[5].data_ptr(), C[6], n_c, d, _ptr(colscale), offset, n_split, _ptr(rs_part), o_part.data_ptr(), s), what)
-    else:
-        check(lib.ssl_softmax_gemm(R[0].data_ptr(), n_r, C[0].data_ptr(), C[1].data_ptr(), n_c, d, _ptr(colscale), offset, n_split,
-                                   _ptr(rs_part), o_part.data_ptr(), s), what)
-
-
 class _DenseLseFn(torch.autograd.Function):
     """mean_b log(sum_j exp(a_b . t_j / temp) + eps) for dense a [B, d], t [n, d] (both receive gradients), without the
     [B, n] logits: forward = the contraction with R = a log2e / temp, C = t; backward w.r.t. a is its O output, w.r.t. t
@@ -1014,40 +990,39 @@ class _DenseLseFn(torch.autograd.Function):
         _require_cuda(t, 'table')
         a, t = a.detach().contiguous().float(), t.detach().contiguous().float()
         (B, d), n = a.shape, t.shape[0]
-        use_tc = USE_TENSOR_CORES and d in (32, 64)
-        A = _raw_operand(a, LOG2E / temp, use_tc)
-        T = _raw_operand(t, 1.0, use_tc)
+        kind = contraction_kind(d, 0.0, raw=True)
         f = dict(device=a.device, dtype=torch.float32)
-        n_split = choose_split((B + 127) // 128, T[6] // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
-        rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
         rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
         with torch.cuda.device(a.device):
             s = _stream(a)
-            with _timed('nce_gemm_fwd', dict(B=B, n=n, dim=d, tc=use_tc)):
-                _gemm(use_tc, A, B, T, n, d, None, 0.0, n_split, rs_part, o_part, s, 'softmax_gemm(lse fwd)')
+            # raw rows (norm_mode 3) with the copies of either role: a and t swap roles in the backward
+            A = _operand(Rows.constant(a), None, 3, LOG2E / temp, s, kind, streamed=True, npad=max(64, ceil_to(B, 64)))
+            T = _operand(Rows.constant(t), None, 3, 1.0, s, kind, streamed=True, npad=max(64, ceil_to(n, 64)))
+            n_split = _n_split(A, T)
+            rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
+            _contract(A, T, None, 0.0, n_split, rs_part, o_part, s)
             check(lib.ssl_lse_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, eps, rowsum.data_ptr(), obar.data_ptr(),
                                        loss_b.data_ptr(), s), 'ssl_lse_finalize')
             check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0 / B, out.data_ptr(), s), 'ssl_sum')
-        ctx.pack = (A, T, B, n, d, temp, use_tc, rowsum, obar)
+        ctx.pack = (A, T, B, n, d, temp, rowsum, obar)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        A, T, B, n, d, temp, use_tc, rowsum, obar = ctx.pack
+        A, T, B, n, d, temp, rowsum, obar = ctx.pack
         g = g.contiguous()
         ga = gt = None
         if ctx.needs_input_grad[0]:
             ga = obar * (g * (1.0 / (B * temp)))                 # d/da_b = softmax-weighted table average / (B temp)
         if ctx.needs_input_grad[1]:
             f = dict(device=g.device, dtype=torch.float32)
-            colscale = torch.zeros(A[6], **f)
-            n_split = choose_split((n + 127) // 128, A[6] // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
+            colscale = torch.zeros(A.npad, **f)
+            n_split = _n_split(T, A)
             dt_part = torch.empty(n_split, n, d, **f)
             with torch.cuda.device(g.device):
                 s = _stream(g)
                 check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), 1.0 / B, colscale.data_ptr(), s), 'ssl_nce_colscale')
-                with _timed('nce_gemm_bwd', dict(B=B, n=n, dim=d, tc=use_tc)):
-                    _gemm(use_tc, T, n, A, B, d, colscale, 0.0, n_split, None, dt_part, s, 'softmax_gemm(lse bwd)')
+                _contract(T, A, colscale, 0.0, n_split, None, dt_part, s)
             gt = dt_part[0] if n_split == 1 else dt_part.sum(0)
         return ga, gt, None, None
 
@@ -1058,41 +1033,15 @@ def dense_logsumexp_mean(a: torch.Tensor, table: torch.Tensor, temp: float, eps:
 
 # ---- DirectAU: alignment / uniformity on unit rows (loss_utils.py:75-86) -----------------------------------
 
-def _unit_rows(e: Rows, idx, alpha: float, streamed: bool, use_tc: bool, f16: bool = False):
-    """F.normalize of the gathered rows e[idx] (norm_mode 2), scaled by ``alpha``; with the operand copies the
-    contraction reads when asked (``streamed``: the C side needs the transposed copies as well, except for ``f16``, the
-    3xFP16 contraction, which reads the row-major fp16 hi / lo parts in both roles)."""
-    dev, d, B = e.base.device, e.dim, idx.numel()
-    Bp = ceil_to(B, 64)
-    f = dict(device=dev, dtype=torch.float32)
-    out, rinv = torch.empty(Bp, d, **f), torch.empty(B, **f)
-    hi = lo = thi = tlo = out_t = None
-    if f16:
-        hi, lo = torch.empty(Bp, d, device=dev, dtype=torch.float16), torch.empty(Bp, d, device=dev, dtype=torch.float16)
-        with torch.cuda.device(dev):
-            check(lib.ssl_rows_normalize_f16x3(e.ptr, e.stride, idx.data_ptr(), B, d, 2, alpha, out.data_ptr(), rinv.data_ptr(),
-                                               hi.data_ptr(), lo.data_ptr(), _stream(e.base)), 'ssl_rows_normalize_f16x3(unit)')
-        return out, rinv, (hi, lo, thi, tlo, out_t)
-    if use_tc:
-        hi, lo = torch.empty(Bp, d, **f), torch.empty(Bp, d, **f)
-        if streamed:
-            thi, tlo = torch.empty(d, Bp, **f), torch.empty(d, Bp, **f)
-    elif streamed:
-        out_t = torch.empty(Bp // 64, d, 64, **f)
-    with torch.cuda.device(dev):
-        check(lib.ssl_rows_normalize(e.ptr, e.stride, idx.data_ptr(), B, d, 2, alpha, out.data_ptr(), _ptr(out_t), rinv.data_ptr(),
-                                     _ptr(hi), _ptr(lo), _ptr(thi), _ptr(tlo), Bp, _stream(e.base)), 'ssl_rows_normalize(unit)')
-    return out, rinv, (hi, lo, thi, tlo, out_t)
-
-
 def _align_fwd(x: Rows, y: Rows, ix, iy):
     """alignment(x, y, alpha=2) = mean_b |x^_b - y^_b|^2 (loss_utils.py:75-79)."""
     dev, d, B = x.base.device, x.dim, ix.numel()
-    xh, rx, _ = _unit_rows(x, ix, 1.0, False, False)
-    yh, ry, _ = _unit_rows(y, iy, 1.0, False, False)
     loss_b, out = torch.empty(B, device=dev), torch.empty((), device=dev)
     with torch.cuda.device(dev):
         s = _stream(x.base)
+        # F.normalize (norm_mode 2): hat and rinv, the FFMA kernel's resident operand
+        xo, yo = _operand(x, ix, 2, 1.0, s, 'ffma'), _operand(y, iy, 2, 1.0, s, 'ffma')
+        xh, yh, rx, ry = xo.hat, yo.hat, xo.rinv, yo.rinv
         check(lib.ssl_align_fwd(xh.data_ptr(), yh.data_ptr(), B, d, loss_b.data_ptr(), s), 'ssl_align_fwd')
         check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0 / B, out.data_ptr(), s), 'ssl_sum')
     return out, (x, y, ix, iy, xh, yh, rx, ry)
@@ -1120,43 +1069,27 @@ def _uniform_fwd(x: Rows, ix):
         raise ValueError('uniformity needs at least 2 rows')
     f = dict(device=dev, dtype=torch.float32)
     pair_sum, w, total = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty((), **f)
-    if B < 256:
-        # The contraction's pair_sum_i = rowsum_i - e_ii cancels when the off-diagonal sum is small next to e_ii = 1
-        # (B = 2-3, near-antipodal rows).  Below 256 rows the pairs are summed directly from x^_i - x^_j instead.
-        c, rinv, _ = _unit_rows(x, ix, 1.0, False, False)
-        with torch.cuda.device(dev):
-            s = _stream(x.base)
-            check(lib.ssl_uniform_pairs(c.data_ptr(), B, d, pair_sum.data_ptr(), w.data_ptr(), s), 'ssl_uniform_pairs')
-            check(lib.ssl_sum(pair_sum.data_ptr(), B, 1.0, total.data_ptr(), s), 'ssl_sum')
-        out = torch.log(total / float(B * (B - 1)))
-        return out, (x, ix, c, rinv, w, total)
-    Bp = ceil_to(B, 64)
-    # from 256 rows on the pair sum is >> e_ii, so removing e_ii loses little and the 3xTF32 contraction (1e-6) suffices
-    use_tc = USE_TENSOR_CORES and d in (32, 64)
-    off = 4.0 * LOG2E
-    f16 = use_tc and f16x3_applies(off)
-    r, _, (r_hi, r_lo, _, _, _) = _unit_rows(x, ix, off, False, use_tc, f16)
-    c, rinv, (c_hi, c_lo, c_thi, c_tlo, c_t) = _unit_rows(x, ix, 1.0, True, use_tc, f16)
-    n_split = choose_split((B + 127) // 128, Bp // 64, slots=NUM_SM if use_tc else 2 * NUM_SM, prefer_few=use_tc)
-    rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
     with torch.cuda.device(dev):
         s = _stream(x.base)
-        with _timed('nce_gemm_fwd', dict(B=B, n=B, dim=d, tc=use_tc)):
-            if f16:
-                check(lib.ssl_softmax_gemm_f16x3(r_hi.data_ptr(), r_lo.data_ptr(), B, c_hi.data_ptr(), c_lo.data_ptr(), B, d, None, off,
-                                                 n_split, rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm_f16x3(uniformity)')
-            elif use_tc:
-                check(lib.ssl_softmax_gemm_tf32x3(r_hi.data_ptr(), r_lo.data_ptr(), B, c_hi.data_ptr(), c_lo.data_ptr(), c_thi.data_ptr(),
-                                                  c_tlo.data_ptr(), Bp, B, d, None, off, n_split, rs_part.data_ptr(), o_part.data_ptr(), s),
-                      'ssl_softmax_gemm_tf32x3(uniformity)')
-            else:
-                check(lib.ssl_softmax_gemm(r.data_ptr(), B, c.data_ptr(), c_t.data_ptr(), B, d, None, off, n_split,
-                                           rs_part.data_ptr(), o_part.data_ptr(), s), 'ssl_softmax_gemm(uniformity)')
-        check(lib.ssl_uniform_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, r.data_ptr(), c.data_ptr(), off,
-                                       pair_sum.data_ptr(), w.data_ptr(), s), 'ssl_uniform_finalize')
+        if B < 256:
+            # The contraction's pair_sum_i = rowsum_i - e_ii cancels when the off-diagonal sum is small next to e_ii = 1
+            # (B = 2-3, near-antipodal rows).  Below 256 rows the pairs are summed directly from x^_i - x^_j instead.
+            c = _operand(x, ix, 2, 1.0, s, 'ffma')
+            check(lib.ssl_uniform_pairs(c.hat.data_ptr(), B, d, pair_sum.data_ptr(), w.data_ptr(), s), 'ssl_uniform_pairs')
+        else:
+            # from 256 rows on the pair sum is >> e_ii, so removing e_ii loses little and an fp32-grade contraction suffices
+            off = 4.0 * LOG2E
+            kind = contraction_kind(d, off)
+            r = _operand(x, ix, 2, off, s, kind)
+            c = _operand(x, ix, 2, 1.0, s, kind, streamed=True)
+            n_split = _n_split(r, c)
+            rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
+            _contract(r, c, None, off, n_split, rs_part, o_part, s)
+            check(lib.ssl_uniform_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, r.hat.data_ptr(), c.hat.data_ptr(), off,
+                                           pair_sum.data_ptr(), w.data_ptr(), s), 'ssl_uniform_finalize')
         check(lib.ssl_sum(pair_sum.data_ptr(), B, 1.0, total.data_ptr(), s), 'ssl_sum')
     out = torch.log(total / float(B * (B - 1)))                 # total counts every unordered pair twice
-    return out, (x, ix, c, rinv, w, total)
+    return out, (x, ix, c.hat, c.rinv, w, total)
 
 
 def _uniform_bwd(pack, g):

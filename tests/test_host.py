@@ -93,6 +93,23 @@ def test_choose_split_fills_waves():
     assert choose_split(200, 64, slots=132, prefer_few=True) == 3 and choose_split(1, 1, slots=132, prefer_few=True) == 1
 
 
+@pytest.mark.parametrize('use_tc', [True, False])
+def test_contraction_kind_table(use_tc, monkeypatch):
+    """The InfoNCE contraction kernel the engine picks (the rule test_gpu_model_paths._expected asserts on the GPU): FFMA off
+    the tensor cores or at d not in {32, 64}; 3xTF32 for raw rows or an offset above 16; else 3xFP16."""
+    from sslrec_b200 import engine as E
+    monkeypatch.setattr(E, 'USE_TENSOR_CORES', use_tc)
+    above = float(np.nextafter(np.float64(E.F16X3_MAX_OFFSET), np.inf))
+    for d in (16, 32, 48, 64, 128):
+        for off in (0.0, 7.2, 16.0, above):
+            for raw in (False, True):
+                want = ('ffma' if not use_tc or d not in (32, 64) else
+                        'tf32x3' if raw or off > 16.0 else 'f16x3')
+                assert E.contraction_kind(d, off, raw) == want, (d, off, raw)
+    assert E.contraction_kind(64, E.LOG2E / 0.2) == ('f16x3' if use_tc else 'ffma')       # InfoNCE at tau = 0.2
+    assert E.contraction_kind(64, E.LOG2E / 0.05) == ('tf32x3' if use_tc else 'ffma')     # tau below 0.0902
+
+
 def test_device_side_components_fail_loudly_without_cuda():
     """No host fallback: the device loader, the native k-means and the DirectAU losses refuse CPU inputs."""
     from sslrec_b200 import loss_utils as LU
