@@ -470,6 +470,22 @@ SSL_API int ssl_kmeans_iter(const float *x, int64_t stride, int64_t n, int32_t d
 SSL_API int ssl_sample_negs(const int64_t *users, int64_t n_pairs, const int32_t *trn_rowptr, const int32_t *trn_cols,
                     int64_t n_item, uint64_t seed, uint32_t epoch, int64_t *negs, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * a22  Ordered scatter of batch rows into a gradient sink (optional key train.deterministic): the
+ *   backward of the batch-row gathers of loss_utils.py:7-10 (BPR), :30-51 (InfoNCE rows) and :75-86
+ *   (alignment / uniformity), and of the torch indexing users[ancs] / items[poss] / items[negs] of
+ *   hccf.py:94 and users[ancs], G_u[ancs], G_i[poss] of lightgcl.py:117-121, in a fixed order.
+ *   stage [n_pos, dim] contiguous: row p = the contribution of batch position p; ids [n_pos] the sink
+ *   row of each position (a negative id: the position is skipped); order [n_pos] the stable ascending
+ *   argsort of ids.  For every row r addressed by some position p1 < p2 < ... (in position order):
+ *     sink[r * stride + k] = sink[r * stride + k] + (((c_p1[k] + c_p2[k]) + c_p3[k]) + ...)
+ *   with plain fp32 adds, each sink row read and written once (no atomics): bit-reproducible
+ *   (csrc/ordered_scatter.cuh).  stride >= dim (a view of an interleaved [N, V, dim] sink has stride V * dim);
+ *   n_pos = 0 is a no-op (stage, ids and order may then be NULL).
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_scatter_rows_ordered(const float *stage, const int64_t *ids, const int64_t *order, int64_t n_pos, int32_t dim,
+                             float *sink, int64_t stride, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

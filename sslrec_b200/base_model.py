@@ -102,6 +102,9 @@ class BaseModel(nn.Module):
         """Attach a parallel.RowShard.  When it row-shards the propagation, the flat [N, d] parameter table moves into a
         shared table (every rank maps every peer's replica) so the sharded Adam can store the rows it updates straight
         into the peers' replicas; rank 0's values are broadcast so all replicas start identical."""
+        from . import engine as E
+        if comm is not None and E.deterministic():
+            raise RuntimeError('train.deterministic is single-GPU: a row-sharded model sums its partials across GPUs in an order of its own')
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

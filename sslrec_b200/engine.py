@@ -272,8 +272,14 @@ class Rows:
     def dense(self) -> torch.Tensor:
         """A strided torch view of the referenced rows (for inspection / tests)."""
         self.require_whole('Rows.dense()')
-        b = self.base.view(-1, self.n_views, self.dim)
-        return b[self.off:self.off + self.n, self.v, :]
+        return self._view()
+
+    def _view(self) -> torch.Tensor:
+        return self.base.view(-1, self.n_views, self.dim)[self.off:self.off + self.n, self.v, :]
+
+    def take(self, idx: torch.Tensor) -> torch.Tensor:
+        """The rows at ``idx`` as a contiguous [len(idx), dim] tensor (a restricted view holds them: its marked rows are the batch's)."""
+        return self._view().index_select(0, idx)
 
     @staticmethod
     def constant(t: torch.Tensor) -> 'Rows':
@@ -707,6 +713,88 @@ def _i64(t: torch.Tensor, device) -> torch.Tensor:
     return t
 
 
+# ---- train.deterministic: batch rows added into their sinks in a fixed order ------------------------------------------
+
+DETERMINISTIC: Optional[bool] = None     # tests set it; None = the optional key train.deterministic of the config
+
+
+def deterministic() -> bool:
+    """The one switch of the ordered mode (optional key ``train.deterministic``, INTEGRATION §2).  On: every loss backward whose
+    ids can repeat has its loss kernel write each position's contribution c_p into a stage (identity ids, one add per element)
+    and adds the stage into the sink with ``ssl_scatter_rows_ordered`` (sink[r] + ((c_p1 + c_p2) + ...), positions in order),
+    instead of adding c_p with float atomics in whatever order the warps run; ``rows_at`` gathers with the same ordered
+    backward.  A training step is then a pure function of (parameters, optimizer state, batch, seeds).  Single GPU only."""
+    if DETERMINISTIC is not None:
+        return bool(DETERMINISTIC)
+    from .config import configs
+    return bool(configs.get('train', {}).get('deterministic', False))
+
+
+def _memo(t: torch.Tensor, name: str, fn):
+    """fn(t), kept on ``t`` while its contents are unchanged (``_version``): an index list is argsorted once per step however
+    many terms scatter by it.  Values computed inside a CUDA-graph capture are kept apart from eager ones, so the graph
+    recomputes at every replay what it captured."""
+    stamp = (t._version, torch.cuda.is_current_stream_capturing())
+    memo = getattr(t, '_ssl_memo', None)
+    if memo is None or memo[0] != stamp:
+        memo = t._ssl_memo = (stamp, {})
+    if name not in memo[1]:
+        memo[1][name] = fn(t)
+    return memo[1][name]
+
+
+def _stage(n: int, d: int, dev) -> torch.Tensor:
+    """[n, d] stage of per-position contributions.  Filled with -0.0, the exact additive identity (+0.0 + -0.0 is +0.0), so
+    the one add a loss kernel makes to each element leaves exactly its c_p there."""
+    return torch.full((n, d), -0.0, device=dev, dtype=torch.float32)
+
+
+def scatter_rows_ordered(stage: torch.Tensor, ids: torch.Tensor, sink_ptr: int, sink_stride: int) -> None:
+    """sink row ids[p] += stage[p] for every position p, in the order of ``ssl_scatter_rows_ordered`` (positions with a negative
+    id skipped).  ``stage`` [P, d] contiguous fp32, ``ids`` [P] int64 on its device; the sink is addressed as sink_ptr + 4 *
+    (row * sink_stride + k)."""
+    order = _memo(ids, 'order', lambda t: torch.argsort(t, stable=True))
+    with torch.cuda.device(stage.device):
+        check(lib.ssl_scatter_rows_ordered(stage.data_ptr(), ids.data_ptr(), order.data_ptr(), ids.numel(), stage.shape[1], sink_ptr,
+                                           sink_stride, _stream(stage)), 'ssl_scatter_rows_ordered')
+
+
+def _scatter_blocks(stage: torch.Tensor, parts) -> None:
+    """Scatter consecutive blocks of ``stage``, one per part (ids, sink pointer, sink stride).  Two parts that address the same
+    sink (SimGCL's view-linear sinks make an InfoNCE term's e1 and e2 the same rows) are ONE scatter over their concatenated
+    positions; otherwise one scatter per part, in order."""
+    if len(parts) == 2 and parts[0][1:] == parts[1][1:]:
+        ids = parts[0][0] if parts[0][0] is parts[1][0] else None
+        both = _memo(ids, 'twice', lambda t: torch.cat([t, t])) if ids is not None else torch.cat([parts[0][0], parts[1][0]])
+        parts = [(both,) + tuple(parts[0][1:])]
+    row = 0
+    for ids, ptr, stride in parts:
+        scatter_rows_ordered(stage[row:row + ids.numel()], ids, ptr, stride)
+        row += ids.numel()
+
+
+class _RowsAtFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, table, ids):
+        ctx.shape, ctx.ids = table.shape, ids
+        return table.index_select(0, ids)
+
+    @staticmethod
+    def backward(ctx, g):
+        sink = torch.zeros(ctx.shape, device=g.device, dtype=torch.float32)
+        scatter_rows_ordered(g.contiguous(), ctx.ids, sink.data_ptr(), sink.stride(0))          # c_p = g[p]
+        return sink, None
+
+
+def rows_at(table: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
+    """``table[ids]`` (the batch gathers of hccf.py:94 and lightgcl.py:117-121).  Under ``deterministic()`` its backward adds
+    the gathered rows' gradients into a zeroed table gradient with the ordered scatter instead of torch's index backward."""
+    if not deterministic():
+        return table[ids]
+    _require_cuda(table, 'gathered table')
+    return _RowsAtFn.apply(table, _i64(ids, table.device))
+
+
 def _tokens(*rows: Rows) -> List[torch.Tensor]:
     seen, out = set(), []
     for r in rows:
@@ -730,8 +818,23 @@ def _bpr_fwd(users: Rows, items: Rows, ancs, poss, negs):
     return out, coef
 
 
-def _bpr_bwd(users: Rows, items: Rows, ancs, poss, negs, coef, g):
+def _bpr_bwd(users: Rows, items: Rows, ancs, poss, negs, coef, g, distinct: bool = False):
+    """``distinct``: the caller's ids never repeat (every sink element gets one add), so the atomic kernel is order-fixed as it is."""
     g = g.contiguous()
+    if not distinct and deterministic():
+        # the kernel on the gathered rows with identity ids computes the same c_p into stages; users are positions ancs[0..B),
+        # items poss[0..B) then negs[0..B) as positions B..2B of one scatter
+        B, d = ancs.numel(), users.dim
+        item_ids = torch.cat([poss, negs])
+        u, i = users.take(ancs), items.take(item_ids)
+        su, si = _stage(B, d, g.device), _stage(2 * B, d, g.device)
+        ar = torch.arange(B, device=g.device)
+        with torch.cuda.device(g.device):
+            check(lib.ssl_bpr_bwd(u.data_ptr(), d, i.data_ptr(), d, ar.data_ptr(), ar.data_ptr(), (ar + B).data_ptr(), B, d, coef.data_ptr(),
+                                  g.data_ptr(), 1.0, su.data_ptr(), d, si.data_ptr(), d, _stream(g)), 'ssl_bpr_bwd')
+        scatter_rows_ordered(su, ancs, users.grad_ptr(), users.grad_stride)
+        scatter_rows_ordered(si, item_ids, items.grad_ptr(), items.grad_stride)
+        return
     with torch.cuda.device(g.device):
         check(lib.ssl_bpr_bwd(users.ptr, users.stride, items.ptr, items.stride, ancs.data_ptr(), poss.data_ptr(),
                               negs.data_ptr(), ancs.numel(), users.dim, coef.data_ptr(), g.data_ptr(), 1.0,
@@ -871,9 +974,10 @@ def _contract(R: Operand, C: Operand, colscale, offset: float, n_split: int, row
               f'{name}({"bwd" if bwd else "fwd"})')
 
 
-def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, deno_eps, live=None):
+def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, deno_eps, live=None, distinct=False):
     """``live``: optional int64 DEVICE scalar; only the first ``*live`` of the ``idx`` rows are anchors (a padded list of
-    capacity idx.numel(), see ``dense_infonce_spec_nodes_mean_dev``).  Shapes and n_split then depend on the capacity only."""
+    capacity idx.numel(), see ``dense_infonce_spec_nodes_mean_dev``).  Shapes and n_split then depend on the capacity only.
+    ``distinct``: the ids of ``idx`` never repeat (see ``_bpr_bwd``)."""
     dev = table.base.device
     table.require_whole('an InfoNCE table operand')
     d, B = table.dim, idx.numel()
@@ -909,11 +1013,32 @@ def _nce_fwd(e1: Rows, e2: Rows, table: Rows, idx, idx2, tau, norm_mode, mean, d
             check(lib.ssl_sum_live(loss_b.data_ptr(), B, live.data_ptr(), 1.0, out.data_ptr(), s), 'ssl_sum_live')
         else:
             check(lib.ssl_sum(loss_b.data_ptr(), B, (1.0 / B) if mean else 1.0, out.data_ptr(), s), 'ssl_sum')
-    return out, (e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live)
+    return out, (e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live, distinct)
+
+
+def _nce_bwd_rows_ordered(saved, g, g1, g2, scale, s):
+    """The row gradients of an InfoNCE term under ``deterministic()``: the row kernel with identity ids into a stage of one block
+    per sink ([g1 positions; g2 positions]), then the ordered scatter.  Count-bounded (``live``): positions b >= *live get id -1."""
+    e1, e2, _, idx, tau, _, a, p, _, _, obar, _, _, live, _ = saved
+    B, d = idx.numel(), a.hat.shape[1]
+    sinks = [(ptr, rows.grad_stride) for ptr, rows in ((g1, e1), (g2, e2)) if ptr is not None]
+    stage = _stage(len(sinks) * B, d, g.device)
+    s1 = stage.data_ptr() if g1 is not None else None
+    s2 = stage[B if g1 is not None else 0:].data_ptr() if g2 is not None else None
+    ar = torch.arange(B, device=g.device)
+    if live is not None:
+        check(lib.ssl_nce_bwd_rows_live(a.hat.data_ptr(), p.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), p.rinv.data_ptr(),
+                                        ar.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, s1, d, s2, d, s), 'ssl_nce_bwd_rows_live')
+        ids = torch.where(ar < live, idx, -1)
+    else:
+        check(lib.ssl_nce_bwd_rows(a.hat.data_ptr(), p.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), p.rinv.data_ptr(),
+                                   ar.data_ptr(), B, d, tau, g.data_ptr(), scale, s1, d, s2, d, s), 'ssl_nce_bwd_rows')
+        ids = idx
+    _scatter_blocks(stage, [(ids, ptr, stride) for ptr, stride in sinks])
 
 
 def _nce_bwd(saved, g):
-    e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live = saved
+    e1, e2, table, idx, tau, mean, a, p, t, rowsum, obar, full_table, comm, live, distinct = saved
     dev, d = g.device, table.dim
     B, n = idx.numel(), table.n
     g = g.contiguous()
@@ -927,7 +1052,9 @@ def _nce_bwd(saved, g):
             # own rows' dense gradient goes to a compact block that is all-gathered and added to the sink
             local_dt = torch.zeros(comm.side_block(full_table.n), d, **f)
             gt, gt_stride = local_dt.data_ptr(), d
-        if live is not None and (g1 is not None or g2 is not None):        # rows b < live only, mean over live
+        if (g1 is not None or g2 is not None) and not distinct and deterministic():
+            _nce_bwd_rows_ordered(saved, g, g1, g2, scale, s)
+        elif live is not None and (g1 is not None or g2 is not None):        # rows b < live only, mean over live
             check(lib.ssl_nce_bwd_rows_live(a.hat.data_ptr(), p.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), p.rinv.data_ptr(),
                                             idx.data_ptr(), B, live.data_ptr(), d, tau, g.data_ptr(), 1.0, g1, e1.grad_stride, g2, e2.grad_stride, s),
                   'ssl_nce_bwd_rows_live')
@@ -1047,18 +1174,24 @@ def _align_fwd(x: Rows, y: Rows, ix, iy):
     return out, (x, y, ix, iy, xh, yh, rx, ry)
 
 
-def _align_bwd(pack, g):
+def _align_bwd(pack, g, distinct: bool = False):
+    """``distinct``: see ``_bpr_bwd``.  Ordered: x's and y's positions are one block each of a stage (one scatter when they
+    address the same sink)."""
     x, y, ix, iy, xh, yh, rx, ry = pack
     B, d = ix.numel(), x.dim
     g = g.contiguous()
     c = 2.0 / B                                                # d/dx^ mean |x^ - y^|^2 = 2 (x^ - y^) / B
+    sides = [(rows, idx, a, b, ri) for (rows, idx, a, b, ri) in ((x, ix, xh, yh, rx), (y, iy, yh, xh, ry)) if rows.grad_ptr() is not None]
+    ordered = not distinct and deterministic()
+    stage = _stage(len(sides) * B, d, g.device) if ordered else None
     with torch.cuda.device(g.device):
         s = _stream(g)
-        for (rows, idx, a, b, ri) in ((x, ix, xh, yh, rx), (y, iy, yh, xh, ry)):
-            gp = rows.grad_ptr()
-            if gp is not None:
-                check(lib.ssl_unit_rows_bwd(a.data_ptr(), ri.data_ptr(), idx.data_ptr(), B, d, a.data_ptr(), c, b.data_ptr(), -c,
-                                            g.data_ptr(), 1.0, gp, rows.grad_stride, s), 'ssl_unit_rows_bwd(align)')
+        for k, (rows, idx, a, b, ri) in enumerate(sides):
+            out, stride, ids = (stage[k * B:].data_ptr(), d, None) if ordered else (rows.grad_ptr(), rows.grad_stride, idx.data_ptr())
+            check(lib.ssl_unit_rows_bwd(a.data_ptr(), ri.data_ptr(), ids, B, d, a.data_ptr(), c, b.data_ptr(), -c,
+                                        g.data_ptr(), 1.0, out, stride, s), 'ssl_unit_rows_bwd(align)')
+    if ordered:
+        _scatter_blocks(stage, [(idx, rows.grad_ptr(), rows.grad_stride) for rows, idx, _, _, _ in sides])
 
 
 def _uniform_fwd(x: Rows, ix):
@@ -1092,15 +1225,21 @@ def _uniform_fwd(x: Rows, ix):
     return out, (x, ix, c.hat, c.rinv, w, total)
 
 
-def _uniform_bwd(pack, g):
+def _uniform_bwd(pack, g, distinct: bool = False):
+    """``distinct``: see ``_bpr_bwd``."""
     x, ix, c, rinv, w, total = pack
     gp = x.grad_ptr()
     if gp is None:
         return
     coef = (g * 8.0 / total).contiguous()                       # d total / d x^_i = 8 sum_{j != i} e_ij x^_j
+    ordered = not distinct and deterministic()
+    stage = _stage(ix.numel(), x.dim, g.device) if ordered else None
+    out, stride, ids = (stage.data_ptr(), x.dim, None) if ordered else (gp, x.grad_stride, ix.data_ptr())
     with torch.cuda.device(g.device):
-        check(lib.ssl_unit_rows_bwd(c.data_ptr(), rinv.data_ptr(), ix.data_ptr(), ix.numel(), x.dim, w.data_ptr(), 1.0, None, 0.0,
-                                    coef.data_ptr(), 1.0, gp, x.grad_stride, _stream(g)), 'ssl_unit_rows_bwd(uniformity)')
+        check(lib.ssl_unit_rows_bwd(c.data_ptr(), rinv.data_ptr(), ids, ix.numel(), x.dim, w.data_ptr(), 1.0, None, 0.0,
+                                    coef.data_ptr(), 1.0, out, stride, _stream(g)), 'ssl_unit_rows_bwd(uniformity)')
+    if ordered:
+        scatter_rows_ordered(stage, ix, gp, x.grad_stride)
 
 
 class _AlignFn(torch.autograd.Function):
@@ -1152,7 +1291,7 @@ class _DenseAlignFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        _align_bwd(ctx.pack, g)
+        _align_bwd(ctx.pack, g, distinct=True)
         return ctx.sinks[0](), ctx.sinks[1]()
 
 
@@ -1165,7 +1304,7 @@ class _DenseUniformFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        _uniform_bwd(ctx.pack, g)
+        _uniform_bwd(ctx.pack, g, distinct=True)
         return ctx.sink()
 
 
@@ -1204,15 +1343,15 @@ class _DenseBprFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         users, items_r, ar, coef, su, si, B = ctx.pack
-        _bpr_bwd(users, items_r, ar, ar, ar + B, coef, g)
+        _bpr_bwd(users, items_r, ar, ar, ar + B, coef, g, distinct=True)
         gi = si()
         return su(), gi[:B], gi[B:]
 
 
 class _DenseInfoNceFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, e1, e2, table, idx, idx2, tau, norm_mode, mean, deno_eps, shared_table, live=None):
-        ctx.n_inputs = 10 if live is None else 11
+    def forward(ctx, e1, e2, table, idx, idx2, tau, norm_mode, mean, deno_eps, shared_table, distinct, live=None):
+        ctx.n_inputs = 11 if live is None else 12
         r1, s1 = _dense_rows(e1, ctx.needs_input_grad[0])
         if shared_table:                      # e2 rows are rows of the table itself (spec_nodes)
             rt, st_ = _dense_rows(table, ctx.needs_input_grad[2])
@@ -1220,7 +1359,7 @@ class _DenseInfoNceFn(torch.autograd.Function):
         else:
             r2, s2 = _dense_rows(e2, ctx.needs_input_grad[1])
             rt, st_ = _dense_rows(table, ctx.needs_input_grad[2])
-        out, ctx.saved_pack = _nce_fwd(r1, r2, rt, idx, idx2, tau, norm_mode, mean, deno_eps, live)
+        out, ctx.saved_pack = _nce_fwd(r1, r2, rt, idx, idx2, tau, norm_mode, mean, deno_eps, live, distinct)
         ctx.sinks = (s1, s2, st_, shared_table)
         return out
 
@@ -1242,13 +1381,13 @@ def dense_infonce_loss_sum(e1, e2, all2, temp):
     """cal_infonce_loss(embeds1 [B,d], embeds2 [B,d], all_embeds2 [N,d], temp) -- loss_utils.py:30-39."""
     B = e1.shape[0]
     ar = torch.arange(B, device=e1.device)
-    return _DenseInfoNceFn.apply(e1, e2, all2, ar, ar, float(temp), 0, False, 0.0, False)
+    return _DenseInfoNceFn.apply(e1, e2, all2, ar, ar, float(temp), 0, False, 0.0, False, True)
 
 
 def dense_infonce_spec_nodes_mean(embeds1, embeds2, nodes, temp):
     """cal_infonce_loss_spec_nodes(embeds1 [N,d], embeds2 [N,d], nodes, temp) -- loss_utils.py:42-51."""
     nodes = _i64(nodes, embeds2.device)
-    return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True)
+    return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, False)
 
 
 def unique_ids(idx: torch.Tensor, n_range: int):
@@ -1284,7 +1423,7 @@ def dense_infonce_spec_nodes_mean_dev(embeds1, embeds2, ids, temp):
     found on the device (``unique_ids``), the term runs over the padded list at capacity ids.numel() and every piece is bounded
     by the device count -- no host read, no data-dependent shape, so a CUDA graph can capture it."""
     nodes, count = unique_ids(ids, embeds2.shape[0])
-    return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, count)
+    return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, False, count)
 
 
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------

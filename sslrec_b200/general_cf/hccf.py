@@ -91,7 +91,7 @@ class HCCF(BaseModel):
         embeds, gcn_out, hyper_out = self.forward(self.adj, self.keep_rate)
         users, items = embeds[:self.user_num], embeds[self.user_num:]
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (hccf.py:70-74)
-        terms = {'bpr_loss': cal_bpr_loss(users[ancs], items[poss], items[negs]) / ancs.shape[0],
+        terms = {'bpr_loss': cal_bpr_loss(E.rows_at(users, ancs), E.rows_at(items, poss), E.rows_at(items, negs)) / ancs.shape[0],
                  'reg_loss': reg_params(self) * self.reg_weight,
                  'cl_loss': self._contrast(gcn_out, hyper_out, ancs, poss) * self.cl_weight}
         return terms['bpr_loss'] + terms['reg_loss'] + terms['cl_loss'], terms

@@ -81,7 +81,12 @@ class LightGCL(BaseModel):
             r, c, v = self._ui
             idx = torch.from_numpy(np.vstack([r, c])).to(dev)
             adj = torch.sparse_coo_tensor(idx, torch.from_numpy(v).to(dev), (self.user_num, self.item_num)).coalesce()
-            svd_u, s, svd_v = torch.svd_lowrank(adj, q=self.svd_q)                                 # aug_utils.py:94
+            if E.deterministic():
+                # torch's CUDA sparse products behind svd_lowrank sum in an order that varies from run to run; its host
+                # operators do not.  Once per model, before the first step
+                svd_u, s, svd_v = (t.to(dev) for t in torch.svd_lowrank(adj.cpu(), q=self.svd_q))
+            else:
+                svd_u, s, svd_v = torch.svd_lowrank(adj, q=self.svd_q)                             # aug_utils.py:94
             self.ut, self.vt = svd_u.T.contiguous(), svd_v.T.contiguous()
             self.u_mul_s, self.v_mul_s = svd_u @ torch.diag(s), svd_v @ torch.diag(s)
         return self.ut, self.vt, self.u_mul_s, self.v_mul_s
@@ -114,11 +119,12 @@ class LightGCL(BaseModel):
         user_embeds, item_embeds = self.forward()
         ancs, poss, negs = batch_data
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (lightgcl.py:101-106)
-        bpr_loss = cal_bpr_loss(user_embeds[ancs], item_embeds[poss], item_embeds[negs]) / ancs.shape[0]
-        g_u, g_i = self.G_u[ancs], self.G_i[poss]
+        at = E.rows_at          # table[ids]; under train.deterministic with an ordered backward
+        bpr_loss = cal_bpr_loss(at(user_embeds, ancs), at(item_embeds, poss), at(item_embeds, negs)) / ancs.shape[0]
+        g_u, g_i = at(self.G_u, ancs), at(self.G_i, poss)
         neg_score = E.dense_logsumexp_mean(g_u, user_embeds, self.temp, 1e-8) + E.dense_logsumexp_mean(g_i, item_embeds, self.temp, 1e-8)
-        pos_score = torch.clamp((g_u * user_embeds[ancs]).sum(1) / self.temp, -5.0, 5.0).mean() \
-            + torch.clamp((g_i * item_embeds[poss]).sum(1) / self.temp, -5.0, 5.0).mean()
+        pos_score = torch.clamp((g_u * at(user_embeds, ancs)).sum(1) / self.temp, -5.0, 5.0).mean() \
+            + torch.clamp((g_i * at(item_embeds, poss)).sum(1) / self.temp, -5.0, 5.0).mean()
         cl_loss = -pos_score + neg_score
         reg_loss = reg_params(self) * self.reg_weight
         cl_loss = self.cl_weight * cl_loss

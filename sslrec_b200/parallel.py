@@ -88,6 +88,9 @@ class RowShard:
                  n_user: Optional[int] = None, transport: str = 'auto', multicast='auto', user_bounds=None, item_bounds=None):
         """user_bounds / item_bounds: optional block boundaries [0, ..., n_side] (world + 1 entries each, e.g. from
         ``balanced_bounds`` of the rows' entry counts); default: equal blocks of ceil(n_side / world) rows."""
+        from . import engine as E
+        if E.deterministic():
+            raise RuntimeError('train.deterministic is single-GPU: RowShard sums its partials across GPUs in an order of its own')
         self.dist, self.rank, self.world, self.n = dist, rank, world, n
         self.n_user = n if n_user is None else int(n_user)          # None: one side only (a contiguous block of rows)
         n_item = n - self.n_user

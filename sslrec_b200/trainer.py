@@ -11,6 +11,7 @@ from copy import deepcopy
 import numpy as np
 import torch
 
+from . import engine as E
 from ._lib import check, lib
 from .config import configs
 from .optim import FusedAdam
@@ -66,6 +67,8 @@ class Trainer(object):
         ``float(v)`` for every loss term right after ``cal_loss`` (:66, :72), i.e. 1 + n_terms blocking device
         syncs per step; here the step's scalars are copied device->pinned host asynchronously and summed when
         the copy has landed (one step later), so the host keeps enqueueing while the GPU works."""
+        if self.grad_sync is not None and E.deterministic():
+            raise RuntimeError('train.deterministic is single-GPU: the gradient all-reduce of grad_sync sums in an order of its own')
         train_dataloader = self.data_handler.train_dataloader
         train_dataloader.dataset.sample_negs()
         if hasattr(train_dataloader.sampler, 'set_epoch'):
