@@ -63,6 +63,15 @@ class BaseModel(nn.Module):
             self._retie()
         return out
 
+    # ---- training checkpoint (Trainer.save_checkpoint / load_checkpoint) ---------------------------------
+    def resume_state(self) -> dict:
+        """What a resumed run needs besides ``state_dict()``: the position of the kernel seed stream.  Models with more
+        non-parameter training state extend it.  Tensors are returned on the CPU."""
+        return {'seeds': self._seeds.state_dict()}
+
+    def load_resume_state(self, state: dict) -> None:
+        self._seeds.load_state_dict(state['seeds'])
+
     # ---- runtime shared by the drop-in models ----------------------------------------------------
     def _init_runtime(self, data_handler):
         from . import engine as E

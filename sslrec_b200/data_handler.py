@@ -131,6 +131,15 @@ class HostBatchLoader:
     def __len__(self):
         return (len(self.dataset) + self.batch_size - 1) // self.batch_size
 
+    def state(self) -> dict:
+        """What a resumed run needs to serve the same batches at an epoch boundary.  The permutation and the negatives come from
+        torch's and numpy's global generators, which the checkpoint holds; NCL's flag counter is the loader's own."""
+        return {'epoch_flag_counter': getattr(self.dataset, 'epoch_flag_counter', None)}
+
+    def load_state(self, state: dict) -> None:
+        if state['epoch_flag_counter'] is not None:
+            self.dataset.epoch_flag_counter = int(state['epoch_flag_counter'])
+
     def __iter__(self):
         ds, n = self.dataset, len(self.dataset)
         torch.empty((), dtype=torch.int64).random_()                               # _BaseDataLoaderIter._base_seed
@@ -219,6 +228,18 @@ class DeviceLoader:
 
     def __len__(self):
         return (self._share() + self.batch_size - 1) // self.batch_size
+
+    def state(self) -> dict:
+        """The shuffling generator, the negative-sampling epoch and NCL's flag counter, at an epoch boundary."""
+        if self.world > 1:
+            raise RuntimeError('DeviceLoader.state: a checkpoint is single-GPU (this loader serves one rank of several)')
+        ds = self.dataset
+        return {'generator': self._gen.get_state(), 'epoch': int(ds.epoch), 'epoch_flag_counter': int(ds.epoch_flag_counter)}
+
+    def load_state(self, state: dict) -> None:
+        self._gen.set_state(state['generator'])
+        self.dataset.epoch = int(state['epoch'])
+        self.dataset.epoch_flag_counter = int(state['epoch_flag_counter'])
 
     def __iter__(self):
         perm = torch.randperm(len(self.dataset), device=self.dataset.device, generator=self._gen)

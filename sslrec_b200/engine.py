@@ -14,6 +14,7 @@ gradient is ever materialised per loss term or added by torch.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import functools
 import math
@@ -189,6 +190,23 @@ class SeedStream:
 
     def disable_device(self) -> None:
         self._dev, self._step_vals, self._cursor = None, [], 0
+
+    @contextlib.contextmanager
+    def host_draws(self):
+        """Seeds drawn outside a training step (an evaluation between graph replays) come from the host sequence, as in the
+        eager loop: without this they would be read from the device buffer of the last step, which they do not belong to."""
+        dev, self._dev = self._dev, None
+        try:
+            yield
+        finally:
+            self._dev = dev
+
+    def state_dict(self) -> dict:
+        """The position in the sequence as two plain ints (never a DevSeed): what a training checkpoint stores."""
+        return {'state': int(self.state), 'count': int(self.count)}
+
+    def load_state_dict(self, sd: dict) -> None:
+        self.state, self.count = int(sd['state']), int(sd['count'])
 
     def begin_step(self, n: int) -> None:
         """Draw this step's ``n`` seeds and enqueue their host -> device copy on the current stream."""

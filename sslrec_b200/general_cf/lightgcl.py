@@ -91,6 +91,23 @@ class LightGCL(BaseModel):
             self.u_mul_s, self.v_mul_s = svd_u @ torch.diag(s), svd_v @ torch.diag(s)
         return self.ut, self.vt, self.u_mul_s, self.v_mul_s
 
+    _FACTORS = ('ut', 'vt', 'u_mul_s', 'v_mul_s')
+
+    def resume_state(self) -> dict:
+        """The seed stream and the low-rank factors: recomputing them would give other factors and take other draws from
+        torch's generator (``svd_lowrank``), so a restored model keeps the saved ones and ``_svd`` does not run again."""
+        state = super().resume_state()
+        if self.ut is not None:
+            state['svd'] = {k: getattr(self, k).detach().cpu() for k in self._FACTORS}
+        return state
+
+    def load_resume_state(self, state: dict) -> None:
+        super().load_resume_state(state)
+        svd = state.get('svd')
+        dev = self.user_embeds.device
+        for k in self._FACTORS:
+            setattr(self, k, None if svd is None else svd[k].to(dev))
+
     # ---- forward -----------------------------------------------------------------------------------
     def forward(self, test=False):
         if test and self.E_u is not None:

@@ -42,6 +42,25 @@ class NCL(LightGCN):
                 dst.copy_(src)
             self.user_centroids, self.user2cluster, self.item_centroids, self.item2cluster = old
 
+    _CLUSTERING = ('user_centroids', 'user2cluster', 'item_centroids', 'item2cluster')
+
+    def resume_state(self) -> dict:
+        """The seed stream and the current clustering: a restored model counts as clustered, so ``cal_loss`` and
+        ``graph_pre_step`` re-cluster only on the next flag of the restored loader."""
+        state = super().resume_state()
+        if hasattr(self, 'user2cluster'):
+            state['clustering'] = {k: getattr(self, k).detach().cpu() for k in self._CLUSTERING}
+        return state
+
+    def load_resume_state(self, state: dict) -> None:
+        super().load_resume_state(state)
+        dev = self.user_embeds.device
+        for k in self._CLUSTERING:
+            if 'clustering' in state:
+                setattr(self, k, state['clustering'][k].to(dev))
+            elif hasattr(self, k):
+                delattr(self, k)
+
     def _run(self):
         ctx_layer = self.high_order * 2
         iteration = max(self.layer_num, ctx_layer)                                              # ncl.py:36

@@ -29,12 +29,17 @@ class FusedAdam(torch.optim.Optimizer):
         self._step_dev = torch.full((1,), steps.pop() if steps else 0, dtype=torch.int64, device=device)
         self._dyn = {}
 
-    def disable_device_step(self) -> None:
+    def sync_host_step(self) -> None:
+        """Copy the device step count into every parameter's host ``step`` (device mode keeps running): ``state_dict()`` then
+        holds the count the next step continues from."""
         if self._step_dev is not None:
             n = int(self._step_dev.item())
             for st in self.state.values():
                 if st:
                     st['step'] = n
+
+    def disable_device_step(self) -> None:
+        self.sync_host_step()
         self._step_dev = None
 
     @torch.no_grad()

@@ -5,6 +5,7 @@ same loop: sample_negs, zero_grad, cal_loss, loss.item(), backward, step, per-te
 from __future__ import annotations
 
 import os
+import tempfile
 import time
 from copy import deepcopy
 
@@ -41,6 +42,62 @@ def _summary_writer():
     return SummaryWriter(log_dir='runs')
 
 
+CHECKPOINT_FORMAT = 1         # version of the dict Trainer.save_checkpoint writes
+
+
+def _to_cpu(obj):
+    """A copy of a nest of dicts / lists / tuples with every tensor moved to the CPU."""
+    if isinstance(obj, torch.Tensor):
+        return obj.detach().cpu()
+    if isinstance(obj, dict):
+        return {k: _to_cpu(v) for k, v in obj.items()}
+    if isinstance(obj, (list, tuple)):
+        return type(obj)(_to_cpu(v) for v in obj)
+    return obj
+
+
+def _numpy_rng_state() -> dict:
+    """numpy's global generator as plain values and one tensor, so the checkpoint loads with ``weights_only=True``."""
+    s = np.random.get_state(legacy=False)
+    return {'bit_generator': s['bit_generator'], 'key': torch.from_numpy(s['state']['key'].astype(np.int64)), 'pos': int(s['state']['pos']),
+            'has_gauss': int(s['has_gauss']), 'gauss': float(s['gauss'])}
+
+
+def _set_numpy_rng_state(s: dict) -> None:
+    np.random.set_state({'bit_generator': s['bit_generator'], 'state': {'key': s['key'].numpy().astype(np.uint32), 'pos': s['pos']},
+                         'has_gauss': s['has_gauss'], 'gauss': s['gauss']})
+
+
+def _atomic_save(obj, path: str) -> None:
+    """torch.save to a temporary file in the target's directory, flushed and fsync'ed, then renamed over ``path``: readers see the
+    old file or the new one, never a partial write."""
+    directory = os.path.dirname(os.path.abspath(path))
+    os.makedirs(directory, exist_ok=True)
+    fd, tmp = tempfile.mkstemp(prefix='.' + os.path.basename(path) + '.', suffix='.tmp', dir=directory)
+    try:
+        with os.fdopen(fd, 'wb') as f:
+            torch.save(obj, f)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.unlink(tmp)
+        raise
+    dfd = os.open(directory, os.O_RDONLY)          # the rename itself survives a crash once the directory is on disk
+    try:
+        os.fsync(dfd)
+    finally:
+        os.close(dfd)
+
+
+def _describe_difference(key, saved, now) -> str:
+    if isinstance(saved, dict) and isinstance(now, dict):
+        keys = sorted((k for k in saved.keys() | now.keys() if saved.get(k) != now.get(k)), key=str)
+        return '{}: {}'.format(key, ', '.join(f'{k} saved {saved.get(k)!r}, now {now.get(k)!r}' for k in keys))
+    return f'{key}: saved {saved!r}, now {now!r}'
+
+
 class Trainer(object):
     def __init__(self, data_handler, logger=None, grad_sync=None):
         self.data_handler = data_handler
@@ -48,6 +105,8 @@ class Trainer(object):
         self.grad_sync = grad_sync     # parallel.BatchShard: data-parallel ranks average gradients before the step
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
+        self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
+        self.early_stop_state = None   # train() with patience: {'waited', 'best_epoch', 'best_metric', 'best_state'}
 
     def _scalar(self, tag, value, step):
         if self._writer is None and configs.get('train', {}).get('tensorboard', False):
@@ -104,6 +163,7 @@ class Trainer(object):
         self._scalar('Loss/train', ep_loss / max(steps, 1), epoch_idx)
         if self.logger is not None:
             self.logger.log_loss(epoch_idx, loss_log_dict, save_to_log=configs['train'].get('log_loss', True))
+        self.epoch_done = epoch_idx
         return ep_loss, loss_log_dict
 
     def _graph_step(self, model, batch_data, recluster=False):
@@ -126,36 +186,48 @@ class Trainer(object):
     def train(self, model):
         """trainer.py:86-137: plain run (evaluate every ``test_step`` epochs, then test + save) or, when the YAML
         carries ``patience`` (configurator sets ``early_stop``), tracking of the best first-metric@k[0] with the
-        best ``state_dict`` restored into a freshly built model before the final evaluate / test / save."""
+        best ``state_dict`` restored into a freshly built model before the final evaluate / test / save.
+
+        Optional keys (single GPU): ``train.checkpoint_step: n`` writes a training checkpoint (``save_checkpoint``) to
+        ``checkpoint_path()`` after every n-th epoch; ``train.resume_path: path`` loads one (``load_checkpoint``) and continues at
+        the epoch after it, with the early-stop counters and best state it holds."""
         self.create_optimizer(model)
         cfg = configs['train']
+        start, self.early_stop_state = 0, None
+        if cfg.get('resume_path'):
+            start = self.load_checkpoint(model, cfg['resume_path'])
+        if cfg.get('checkpoint_step'):
+            self._single_gpu(model, 'train.checkpoint_step')       # refused now rather than at the first checkpoint
+            self._train_loader('train.checkpoint_step')
         if not cfg.get('early_stop', False):
-            for epoch_idx in range(cfg['epoch']):
+            for epoch_idx in range(start, cfg['epoch']):
                 self.train_epoch(model, epoch_idx)
                 if epoch_idx % cfg['test_step'] == 0:
                     self.evaluate(model, epoch_idx)
+                self._checkpoint_after(model, epoch_idx)
             self.test(model)
             self.save_model(model)
             return model
         key = configs['test']['metrics'][0]
-        waited, best_epoch, best_metric, best_state = 0, 0, -1e9, None
-        for epoch_idx in range(cfg['epoch']):
-            self.train_epoch(model, epoch_idx)
-            if epoch_idx % cfg['test_step'] != 0:
-                continue
-            score = self.evaluate(model, epoch_idx)[key][0]
-            if score > best_metric:
-                waited, best_epoch, best_metric = 0, epoch_idx, score
-                best_state = deepcopy(model.state_dict())
-                self._log('Validation score increased.  Copying the best model ...')
-            else:
-                waited += 1
-                self._log(f"Early stop counter: {waited} out of {cfg['patience']}")
-            if waited == cfg['patience']:
+        es = self.early_stop_state = self.early_stop_state or {'waited': 0, 'best_epoch': 0, 'best_metric': -1e9, 'best_state': None}
+        for epoch_idx in range(start, cfg['epoch']):
+            if es['waited'] >= cfg['patience']:           # resumed from the checkpoint of the epoch that stopped the run
                 break
-        self._log('Best Epoch {}'.format(best_epoch))
-        if best_state is not None:
-            model = self._rebuild(model, best_state)
+            self.train_epoch(model, epoch_idx)
+            if epoch_idx % cfg['test_step'] == 0:
+                score = self.evaluate(model, epoch_idx)[key][0]
+                if score > es['best_metric']:
+                    es.update(waited=0, best_epoch=epoch_idx, best_metric=score, best_state=deepcopy(model.state_dict()))
+                    self._log('Validation score increased.  Copying the best model ...')
+                else:
+                    es['waited'] += 1
+                    self._log(f"Early stop counter: {es['waited']} out of {cfg['patience']}")
+            self._checkpoint_after(model, epoch_idx)
+            if es['waited'] >= cfg['patience']:
+                break
+        self._log('Best Epoch {}'.format(es['best_epoch']))
+        if es['best_state'] is not None:
+            model = self._rebuild(model, es['best_state'])
         self.evaluate(model)
         self.test(model)
         self.save_model(model)
@@ -207,12 +279,122 @@ class Trainer(object):
         self._log('Load model parameters from {}'.format(path))
         return model
 
+    # ---- training checkpoints: everything a run needs to continue as if it had never stopped ---------------------------
+    def checkpoint_path(self) -> str:
+        """./checkpoint/{model}/{model}-{data}-resume.pth (tune runs: ./checkpoint/{model}/tune/...), the directory of save_model."""
+        model_name, data_name = configs['model']['name'], configs['data']['name']
+        tune = configs.get('tune', {}).get('enable', False)
+        return './checkpoint/{}{}/{}-{}-resume.pth'.format(model_name, '/tune' if tune else '', model_name, data_name)
+
+    def _checkpoint_after(self, model, epoch_idx):
+        n = configs['train'].get('checkpoint_step')
+        if n and (epoch_idx + 1) % n == 0:
+            path = self.save_checkpoint(model, self.checkpoint_path())
+            self._log('Save training checkpoint to {}'.format(path))
+
+    def _single_gpu(self, model, what):
+        if self.grad_sync is not None or getattr(model, 'comm', None) is not None:
+            raise RuntimeError(f'{what}: training checkpoints are single-GPU (a multi-GPU run shards its optimizer and table state)')
+
+    def _train_loader(self, what):
+        """-> (kind, loader) for the train loaders whose position a checkpoint can hold."""
+        from .data_handler import DeviceLoader, HostBatchLoader
+        loader = self.data_handler.train_dataloader
+        if isinstance(loader, HostBatchLoader):
+            return 'host', loader
+        if isinstance(loader, DeviceLoader):
+            return 'device', loader
+        raise RuntimeError(f'{what}: the train loader {type(loader).__name__} does not expose its iterator state, so a resumed run '
+                           'would train on other batches; use the default HostBatchLoader (no train.torch_dataloader) or train.device_loader')
+
+    def _resume_record(self, model, kind):
+        """What a checkpoint must agree on with the run that loads it.  train.epoch, patience, test_step and the test section may
+        differ (a run can be extended)."""
+        t = configs['train']
+        return {'model': configs['model']['name'], 'data': configs['data']['name'], 'user_num': int(model.user_num),
+                'item_num': int(model.item_num), 'model_config': deepcopy(configs['model']), 'optimizer_config': deepcopy(configs['optimizer']),
+                'batch_size': t['batch_size'], 'seed': t.get('seed'), 'loader': kind, 'deterministic': E.deterministic()}
+
+    def save_checkpoint(self, model, path):
+        """Write a training checkpoint at an epoch boundary: parameters, the model's other training state (``resume_state``), the
+        optimizer with its step count, the kernel seed stream, numpy's, torch's and CUDA's global generators, the train loader's
+        position, the last finished epoch, the early-stop state and a record of the run it belongs to.  Every tensor is stored on
+        the CPU.  The file is replaced atomically: a crash while writing leaves the previous checkpoint intact.  Returns ``path``."""
+        self._single_gpu(model, 'save_checkpoint')
+        kind, loader = self._train_loader('save_checkpoint')
+        g = self._graphed
+        if g is not None and g._primed:
+            # the seeds of the graph's first replay are drawn but unused; a resumed run could not draw them again, so this run
+            # drops them too and captures afresh at its next step, as the resumed run does
+            g.close()
+            self._graphed = None
+        self.optimizer.sync_host_step()
+        es = self.early_stop_state
+        ckpt = {
+            'format': CHECKPOINT_FORMAT,
+            'record': self._resume_record(model, kind),
+            'model': _to_cpu(model.state_dict()),
+            'model_resume': _to_cpu(model.resume_state()),
+            'optimizer': _to_cpu(self.optimizer.state_dict()),
+            'rng': {'numpy': _numpy_rng_state(), 'torch': torch.get_rng_state(), 'cuda': [s.cpu() for s in torch.cuda.get_rng_state_all()]},
+            'loader': loader.state(),
+            'trainer': {'epoch': int(self.epoch_done),
+                        'early_stop': None if es is None else {'waited': int(es['waited']), 'best_epoch': int(es['best_epoch']),
+                                                              'best_metric': float(es['best_metric']),
+                                                              'best_state': _to_cpu(es['best_state'])}},
+        }
+        _atomic_save(ckpt, path)
+        return path
+
+    def load_checkpoint(self, model, path) -> int:
+        """Restore a ``save_checkpoint`` file into ``model``, this trainer's optimizer (created if missing), the generators and the
+        train loader.  Raises when the checkpoint belongs to another run (model, data, sizes, the model and optimizer sections,
+        batch size, seed, loader kind, train.deterministic) or to a multi-GPU one.  Returns the epoch to continue at."""
+        self._single_gpu(model, 'load_checkpoint')
+        kind, loader = self._train_loader('load_checkpoint')
+        ckpt = torch.load(path, map_location='cpu', weights_only=True)
+        if not isinstance(ckpt, dict) or ckpt.get('format') != CHECKPOINT_FORMAT:
+            raise ValueError(f'{path}: not a training checkpoint of format {CHECKPOINT_FORMAT} (save_checkpoint writes one)')
+        saved, now = ckpt['record'], self._resume_record(model, kind)
+        diff = [_describe_difference(k, saved.get(k), now[k]) for k in now if saved.get(k) != now[k]]
+        if diff:
+            raise ValueError(f'{path}: the checkpoint belongs to another run: ' + '; '.join(diff))
+        if self._graphed is not None:                  # captured around the old state: the next step captures afresh
+            self._graphed.close()
+            self._graphed = None
+        if not hasattr(self, 'optimizer'):
+            self.create_optimizer(model)
+        model.load_state_dict(ckpt['model'])
+        model.load_resume_state(ckpt['model_resume'])
+        self.optimizer.load_state_dict(ckpt['optimizer'])
+        rng = ckpt['rng']
+        _set_numpy_rng_state(rng['numpy'])
+        torch.set_rng_state(rng['torch'])
+        for i, s in enumerate(rng['cuda'][:torch.cuda.device_count()]):
+            torch.cuda.set_rng_state(s, i)
+        loader.load_state(ckpt['loader'])
+        tr = ckpt['trainer']
+        self.epoch_done = tr['epoch']
+        es = tr['early_stop']
+        if es is not None and es['best_state'] is not None:
+            es['best_state'] = {k: v.to(configs['device']) for k, v in es['best_state'].items()}
+        self.early_stop_state = es
+        self._log('Load training checkpoint from {} (epoch {})'.format(path, self.epoch_done))
+        return self.epoch_done + 1
+
     @torch.no_grad()
     def evaluate(self, model, epoch_idx=None, loader=None, data_type=None):
         """All-rank evaluation: full_predict -> top-max(k) on device (one fused predict_topk call when the model has it and the catalogue
         has at least FUSED_TOPK_MIN_ITEMS items) -> recall / ndcg / precision / mrr on host
         (metrics.py:11-45, :82-127).  Validation split when the handler has one, else the test split
         (trainer.py:139-150)."""
+        seeds = getattr(model, '_seeds', None)
+        if seeds is None:
+            return self._evaluate(model, epoch_idx, loader, data_type)
+        with seeds.host_draws():         # between CUDA-graph replays too, the forward pass takes the next seeds of the host sequence
+            return self._evaluate(model, epoch_idx, loader, data_type)
+
+    def _evaluate(self, model, epoch_idx, loader, data_type):
         model.eval()
         if loader is None:
             if hasattr(self.data_handler, 'valid_dataloader'):
