@@ -486,6 +486,24 @@ SSL_API int ssl_sample_negs(const int64_t *users, int64_t n_pairs, const int32_t
 SSL_API int ssl_scatter_rows_ordered(const float *stage, const int64_t *ids, const int64_t *order, int64_t n_pos, int32_t dim,
                              float *sink, int64_t stride, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * a24  (no counterpart: dynamic negative sampling, optional key train.dns_candidates = M)
+ *   ssl_neg_candidates: cands [n_pairs, M] int64.  cands[b, 0] = negs[b]; cands[b, j >= 1] an item
+ *   drawn uniformly until users[b] has no training interaction with it, with ssl_sample_negs's
+ *   rejection rule and 64-block cap on Philox4x32-10 blocks keyed (seed; b, j, block, "DNSC").  The
+ *   seed is *seed_ptr when seed_ptr is non-null (CUDA-graph replay), else seed.  2 <= M <= 256.
+ *   ssl_neg_select: negs_out[b] = cands[b, j*], j* the candidate with the largest score
+ *   s_j = U[ancs[b]] . I[cands[b, j]], each one sequential fp32 FMA chain over k = 0 .. dim-1; ties
+ *   go to the lowest j, a NaN score never wins, all NaN gives j* = 0 (csrc/hard_negs.cuh).  Rows are
+ *   u_tbl + id * u_stride and i_tbl + id * i_stride (elements; i_tbl is item 0's row).  One writer
+ *   per output, no atomics.  dim <= SSL_MAX_DIM, 2 <= M <= 256.  n_pairs = 0 is a no-op for both.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_neg_candidates(const int64_t *users, const int64_t *negs, int64_t n_pairs, int32_t M, const int32_t *trn_rowptr,
+                               const int32_t *trn_cols, int64_t n_item, uint64_t seed, const uint64_t *seed_ptr, int64_t *cands,
+                               void *stream);
+SSL_API int ssl_neg_select(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
+                           const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, int64_t *negs_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,6 +109,8 @@ def _load():
         'ssl_kmeans_iter': (C.c_int, [vp, i64, i64, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
         'ssl_sample_negs': (C.c_int, [vp, i64, vp, vp, i64, C.c_uint64, C.c_uint32, vp, vp]),
         'ssl_scatter_rows_ordered': (C.c_int, [vp, vp, vp, i64, i32, vp, i64, vp]),
+        'ssl_neg_candidates': (C.c_int, [vp, vp, i64, i32, vp, vp, i64, C.c_uint64, vp, vp, vp]),
+        'ssl_neg_select': (C.c_int, [vp, i64, vp, i64, vp, vp, i64, i32, i32, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export what the header declares

@@ -84,6 +84,30 @@ class BaseModel(nn.Module):
         # optional: data_handler.plan_source(device, row_ranges, side_split) -> GraphPlan builds the CSR plan without a
         # torch sparse COO tensor (BASELINE config 4: 300 M stored entries are generated and sorted on the device)
         self._plan_source = getattr(data_handler, 'plan_source', None)
+        # optional key train.dns_candidates = M (dynamic negative sampling): >= 2 trains each pair on the highest-scored of M
+        # candidates; ``dns_negs`` then holds the selected negatives of the last step (like ``final_embeds``: last step only)
+        self.dns_candidates = E.dns_candidates()
+        self.dns_negs = None
+        if self.dns_candidates > 1 and not self.bpr_negatives:
+            raise ValueError(f'train.dns_candidates: {type(self).__name__} trains without negatives')
+
+    bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates applies)
+
+    def _dns_candidates(self, ancs, negs):
+        """The batch's [B, M] DNS candidates (``engine.neg_candidates``; column 0 = the loader's ``negs``), or None when
+        train.dns_candidates is 1.  Their seed is the last one the step draws, so a DNS step draws every seed of the plain
+        step in the same order."""
+        if self.dns_candidates == 1:
+            return None
+        from . import engine as E
+        rowptr, cols = self._train_csr(ancs.device)
+        return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, self._seeds.next())
+
+    def _dns_select(self, users, items, ancs, cands) -> torch.Tensor:
+        """The highest-scored candidate of every pair on the rows the BPR term reads (``engine.hard_negatives``), kept as ``dns_negs``."""
+        from . import engine as E
+        self.dns_negs = E.hard_negatives(users, items, ancs, cands)
+        return self.dns_negs
 
     def _plan(self, adj=None) -> GraphPlan:
         """CSR plan of an adjacency tensor, built once per (tensor, device)."""
@@ -114,6 +138,8 @@ class BaseModel(nn.Module):
         from . import engine as E
         if comm is not None and E.deterministic():
             raise RuntimeError('train.deterministic is single-GPU: a row-sharded model sums its partials across GPUs in an order of its own')
+        if comm is not None and self.dns_candidates > 1:
+            raise ValueError('train.dns_candidates is single-GPU: a row-sharded model does not select hard negatives')
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

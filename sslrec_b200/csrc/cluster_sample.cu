@@ -28,15 +28,6 @@ __global__ void kmeans_update_kernel(const float *__restrict__ part_sum, const f
 // A user who interacted with every item would never terminate in the reference; here the draw is
 // accepted after 64 blocks (256 rejected draws).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool csr_contains(const int32_t *__restrict__ cols, int lo, int hi, int key) {
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        const int v = __ldg(cols + mid);
-        if (v == key) return true;
-        if (v < key) lo = mid + 1; else hi = mid;
-    }
-    return false;
-}
 
 __global__ void sample_negs_kernel(const int64_t *__restrict__ users, int64_t n_pairs, const int32_t *__restrict__ rowptr,
                                    const int32_t *__restrict__ cols, int64_t n_item, uint64_t seed, uint32_t epoch,
@@ -56,7 +47,7 @@ __global__ void sample_negs_kernel(const int64_t *__restrict__ users, int64_t n_
             if (done) continue;
             // unbiased enough for n_item << 2^32: multiply-shift maps the 32 random bits onto [0, n_item)
             neg = (uint32_t)(((uint64_t)draw[t] * (uint64_t)n_item) >> 32);
-            done = !csr_contains(cols, lo, hi, (int)neg);
+            done = !ssl::csr_contains(cols, lo, hi, (int)neg);
         }
         if (done) break;
     }

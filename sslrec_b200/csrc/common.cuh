@@ -91,6 +91,18 @@ __host__ __device__ __forceinline__ float4 noise_u4_rng(uint64_t seed, uint32_t 
     return make_float4(u01(r.x), u01(r.y), u01(r.z), u01(r.w));
 }
 
+// key in the sorted int32 column list cols[lo, hi) (a training-CSR row)?  Binary search; the negative samplers'
+// rejection test (sample_negs_kernel, hard_negs.cu).
+__device__ __forceinline__ bool csr_contains(const int32_t *__restrict__ cols, int lo, int hi, int key) {
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        const int v = __ldg(cols + mid);
+        if (v == key) return true;
+        if (v < key) lo = mid + 1; else hi = mid;
+    }
+    return false;
+}
+
 // 3xTF32 split: hi = round-to-nearest tf32(x), lo = round-to-nearest tf32(x - hi).  Rounding (not
 // truncating) both parts keeps the residual |x - hi - lo| <= 2^-22 |x| and unbiased.
 __device__ __forceinline__ float tf32_rna(float x) {

@@ -1444,6 +1444,67 @@ def dense_infonce_spec_nodes_mean_dev(embeds1, embeds2, ids, temp):
     return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, False, count)
 
 
+# ---- dynamic negative sampling (optional key train.dns_candidates) ----------------------------------------------------------
+
+DNS_MAX_CANDIDATES = 256
+
+
+def dns_candidates() -> int:
+    """The optional key ``train.dns_candidates`` (INTEGRATION §2): M, the candidates per BPR pair, an integer in [1, 256];
+    1 (the default) is the plain step.  Raises ValueError for any other value."""
+    from .config import configs
+    m = configs.get('train', {}).get('dns_candidates', 1)
+    if isinstance(m, bool) or not isinstance(m, int) or not 1 <= m <= DNS_MAX_CANDIDATES:
+        raise ValueError(f'train.dns_candidates must be an integer in [1, {DNS_MAX_CANDIDATES}], got {m!r}')
+    return m
+
+
+def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torch.Tensor, n_item: int, seed) -> torch.Tensor:
+    """[B, m] int64 negative candidates of the pairs (users[b], ., negs[b]) (``ssl_neg_candidates``): column 0 is ``negs``, the
+    others are drawn uniformly over the items, rejecting the user's training positives (int32 CSR, sorted rows).  A
+    :class:`DevSeed` passes its device word, so a captured step draws with the seed written there before each replay."""
+    dev = trn_cols.device
+    users, negs = _i64(users, dev), _i64(negs, dev)
+    if negs.numel() != users.numel():
+        raise RuntimeError('sslrec_b200: one negative per user')
+    cands = torch.empty(users.numel(), int(m), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ssl_neg_candidates(users.data_ptr(), negs.data_ptr(), users.numel(), int(m), trn_rowptr.data_ptr(), trn_cols.data_ptr(),
+                                     int(n_item), int(seed), getattr(seed, 'ptr', 0) or None, cands.data_ptr(), _stream(cands)),
+              'ssl_neg_candidates')
+    return cands
+
+
+def _score_table(t):
+    """Rows or a [n, d] fp32 tensor with unit column stride -> (pointer of row 0, row stride, dim)."""
+    if isinstance(t, Rows):
+        return t.ptr, t.stride, t.dim
+    _require_cuda(t, 'score table')
+    if t.dim() != 2 or t.stride(1) != 1:
+        raise RuntimeError('sslrec_b200: a score table must be [n, d] with unit column stride')
+    return t.data_ptr(), t.stride(0), t.shape[1]
+
+
+def hard_negatives(users, items, ancs, cands: torch.Tensor) -> torch.Tensor:
+    """[B] int64: for every pair b the candidate cands[b, j] whose score users[ancs[b]] . items[cands[b, j]] is largest
+    (``ssl_neg_select``: one sequential fp32 FMA chain per score, ties to the lowest j, NaN never wins).  ``users`` / ``items``
+    are :class:`Rows` (a restricted view must mark every candidate row) or [n, d] tensors; no gradient flows through it."""
+    u_ptr, u_stride, d = _score_table(users)
+    i_ptr, i_stride, d_i = _score_table(items)
+    if d_i != d:
+        raise RuntimeError('sslrec_b200: user and item rows differ in width')
+    dev = cands.device
+    ancs, cands = _i64(ancs, dev), _i64(cands, dev)
+    B, m = cands.shape
+    if ancs.numel() != B:
+        raise RuntimeError('sslrec_b200: one anchor per row of candidates')
+    out = torch.empty(B, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ssl_neg_select(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), cands.data_ptr(), B, m, d, out.data_ptr(), _stream(out)),
+              'ssl_neg_select')
+    return out
+
+
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------
 
 def _rowgemm(in1, k1, m1, m1_trans, out, n_out, scale=1.0, slope=1.0, accumulate=False, in2=None, k2=0, m2=None, m2_trans=False, pre_ref=None,

@@ -11,6 +11,8 @@ from ..loss_utils import alignment, uniformity
 
 
 class DirectAU(BaseModel):
+    bpr_negatives = False          # alignment / uniformity only: train.dns_candidates > 1 is refused
+
     def __init__(self, data_handler):
         super().__init__(data_handler)
         self.adj = data_handler.torch_adj

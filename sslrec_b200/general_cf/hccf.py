@@ -90,6 +90,9 @@ class HCCF(BaseModel):
         ancs, poss, negs = batch_data
         embeds, gcn_out, hyper_out = self.forward(self.adj, self.keep_rate)
         users, items = embeds[:self.user_num], embeds[self.user_num:]
+        cands = self._dns_candidates(ancs, negs)
+        if cands is not None:
+            negs = self._dns_select(users.detach(), items.detach(), ancs, cands)
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (hccf.py:70-74)
         terms = {'bpr_loss': cal_bpr_loss(E.rows_at(users, ancs), E.rows_at(items, poss), E.rows_at(items, negs)) / ancs.shape[0],
                  'reg_loss': reg_params(self) * self.reg_weight,

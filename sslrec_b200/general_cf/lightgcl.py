@@ -135,6 +135,9 @@ class LightGCL(BaseModel):
         self.is_training = True
         user_embeds, item_embeds = self.forward()
         ancs, poss, negs = batch_data
+        cands = self._dns_candidates(ancs, negs)
+        if cands is not None:
+            negs = self._dns_select(user_embeds.detach(), item_embeds.detach(), ancs, cands)
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (lightgcl.py:101-106)
         at = E.rows_at          # table[ids]; under train.deterministic with an ordered backward
         bpr_loss = cal_bpr_loss(at(user_embeds, ancs), at(item_embeds, poss), at(item_embeds, negs)) / ancs.shape[0]

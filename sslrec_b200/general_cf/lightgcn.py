@@ -58,6 +58,9 @@ class LightGCN(BaseModel):
         ancs, poss, negs = batch_data
         st = self._propagate([self._edge_view(self.keep_rate)])
         self.final_embeds = st.E.view(st.n, st.dim)
+        cands = self._dns_candidates(ancs, negs)
+        if cands is not None:
+            negs = self._dns_select(st.users(0), st.items(0), ancs, cands)
         bpr_loss = cal_bpr_loss(st.users(0), st.items(0), ancs, poss, negs) / ancs.shape[0]
         reg_loss = self.reg_weight * reg_params(self)
         loss = bpr_loss + reg_loss

@@ -82,6 +82,9 @@ class NCL(LightGCN):
         if not getattr(self, '_graph_mode', False) and (not hasattr(self, 'user2cluster') or bool(torch.sum(kmeans_flags) != 0)):
             self._cluster()
         embeds, st = self.forward(self.adj)
+        cands = self._dns_candidates(ancs, negs)
+        if cands is not None:
+            negs = self._dns_select(st.users(0), st.items(0), ancs, cands)
         ctx = self.high_order * 2
         bsz = ancs.shape[0]
         # structure loss (ncl.py:51-58): context (layer 2*high_order) vs ego (layer 0), all ego rows as negatives

@@ -41,11 +41,16 @@ class SGL(LightGCN):
         keep_rate = configs['model']['keep_rate']
         ancs, poss, negs = batch_data
         # views 0, 1: augmented (sgl.py:48-49); view 2: keep_rate 1.0 (sgl.py:50).  View 0 is read at the batch rows only (InfoNCE
-        # anchors); view 2 becomes final_embeds and view 1 is the InfoNCE table, so both are computed at every row
-        v0 = self._aug_view(keep_rate, 0)
-        v0.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, (ancs, 0), (poss, self.user_num), (negs, self.user_num))
-        st = self._propagate([v0, self._aug_view(keep_rate, 1), E.ViewSpec()], n_layers=configs['model']['layer_num'])
+        # anchors); view 2 becomes final_embeds and view 1 is the InfoNCE table, so both are computed at every row.  With
+        # train.dns_candidates the idx=negs term reads view 0 at the selected negatives, so every candidate is a batch row
+        v0, v1 = self._aug_view(keep_rate, 0), self._aug_view(keep_rate, 1)
+        cands = self._dns_candidates(ancs, negs)
+        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
+        v0.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
+        st = self._propagate([v0, v1, E.ViewSpec()], n_layers=configs['model']['layer_num'])
         self.final_embeds = st.E[:, 2, :]
+        if cands is not None:
+            negs = self._dns_select(st.users(2), st.items(2), ancs, cands)
         bsz = ancs.shape[0]
         bpr_loss = cal_bpr_loss(st.users(2), st.items(2), ancs, poss, negs) / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \

@@ -32,11 +32,15 @@ class SimGCL(LightGCN):
         self.is_training = True
         ancs, poss, negs = batch_data
         # views 0, 1: perturbed (simgcl.py:41-42); view 2: clean (simgcl.py:43).  Views 0 (InfoNCE anchors) and 2 (BPR) are
-        # read at the batch rows only, so the last layer computes them there; view 1 is the InfoNCE table (every row)
-        batch_rows = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, (ancs, 0), (poss, self.user_num), (negs, self.user_num))
-        v0, v2 = self._noise_view(0), E.ViewSpec()
-        v0.row_bits = v2.row_bits = batch_rows
-        st = self._propagate([v0, self._noise_view(1), v2], noise_eps=self.eps)
+        # read at the batch rows only, so the last layer computes them there; view 1 is the InfoNCE table (every row).  With
+        # train.dns_candidates the BPR term's negative is chosen on view 2 among the candidates, so they are batch rows too
+        v0, v1, v2 = self._noise_view(0), self._noise_view(1), E.ViewSpec()
+        cands = self._dns_candidates(ancs, negs)
+        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
+        v0.row_bits = v2.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
+        st = self._propagate([v0, v1, v2], noise_eps=self.eps)
+        if cands is not None:
+            negs = self._dns_select(st.users(2), st.items(2), ancs, cands)
         bsz = ancs.shape[0]
         bpr_loss = cal_bpr_loss(st.users(2), st.items(2), ancs, poss, negs) / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \

@@ -103,6 +103,8 @@ class Trainer(object):
         self.data_handler = data_handler
         self.logger = logger
         self.grad_sync = grad_sync     # parallel.BatchShard: data-parallel ranks average gradients before the step
+        if grad_sync is not None and E.dns_candidates() > 1:
+            raise ValueError('train.dns_candidates is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
         self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
@@ -311,9 +313,12 @@ class Trainer(object):
         """What a checkpoint must agree on with the run that loads it.  train.epoch, patience, test_step and the test section may
         differ (a run can be extended)."""
         t = configs['train']
-        return {'model': configs['model']['name'], 'data': configs['data']['name'], 'user_num': int(model.user_num),
-                'item_num': int(model.item_num), 'model_config': deepcopy(configs['model']), 'optimizer_config': deepcopy(configs['optimizer']),
-                'batch_size': t['batch_size'], 'seed': t.get('seed'), 'loader': kind, 'deterministic': E.deterministic()}
+        record = {'model': configs['model']['name'], 'data': configs['data']['name'], 'user_num': int(model.user_num),
+                  'item_num': int(model.item_num), 'model_config': deepcopy(configs['model']), 'optimizer_config': deepcopy(configs['optimizer']),
+                  'batch_size': t['batch_size'], 'seed': t.get('seed'), 'loader': kind, 'deterministic': E.deterministic()}
+        if E.dns_candidates() > 1:          # only then: the records of runs without the key stay as they were
+            record['dns_candidates'] = E.dns_candidates()
+        return record
 
     def save_checkpoint(self, model, path):
         """Write a training checkpoint at an epoch boundary: parameters, the model's other training state (``resume_state``), the
@@ -356,7 +361,8 @@ class Trainer(object):
         if not isinstance(ckpt, dict) or ckpt.get('format') != CHECKPOINT_FORMAT:
             raise ValueError(f'{path}: not a training checkpoint of format {CHECKPOINT_FORMAT} (save_checkpoint writes one)')
         saved, now = ckpt['record'], self._resume_record(model, kind)
-        diff = [_describe_difference(k, saved.get(k), now[k]) for k in now if saved.get(k) != now[k]]
+        diff = [_describe_difference(k, saved.get(k), now.get(k)) for k in list(now) + [k for k in saved if k not in now]
+                if saved.get(k) != now.get(k)]
         if diff:
             raise ValueError(f'{path}: the checkpoint belongs to another run: ' + '; '.join(diff))
         if self._graphed is not None:                  # captured around the old state: the next step captures afresh

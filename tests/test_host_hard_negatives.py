@@ -1,0 +1,120 @@
+"""Dynamic negative sampling (train.dns_candidates) without a GPU: the numpy restatement of ssl_neg_candidates's draws
+(tests/dns_oracle.neg_candidates) against a scalar restatement of the documented rule, its 64-block cap, the float64 selection of
+the oracle, and the key's validation and refusals: values outside [1, 256], DirectAU, a row-sharded model, data-parallel
+gradient sync, and training checkpoints of runs with another M."""
+import types
+
+import numpy as np
+import pytest
+import scipy.sparse as sp
+import torch
+
+import dns_oracle as D
+from oracle import inputs
+from oracle import philox as P
+from test_host_resume import make_run
+
+
+def _csr(rows, cols, n_user, n_item):
+    m = sp.csr_matrix((np.ones(len(rows), np.float32), (rows, cols)), shape=(n_user, n_item))
+    m.sum_duplicates()
+    m.sort_indices()
+    return m.indptr, m.indices
+
+
+def _scalar_candidate(u, b, j, rowptr, cols, n_item, seed):
+    """Candidate j >= 1 of pair b, one draw at a time: word t % 4 of block t // 4 keyed (b, j, block, TAG_DNSC), multiply-shift,
+    rejected while a training positive of u; after 64 blocks the last draw is kept."""
+    pos = set(cols[rowptr[u]:rowptr[u + 1]].tolist())
+    for t in range(256):
+        w = int(P.philox4x32_10(b, j, t // 4, D.TAG_DNSC, seed)[t % 4])
+        c = (w * n_item) >> 32
+        if c not in pos:
+            return c
+    return c
+
+
+def test_candidate_oracle_matches_a_scalar_restatement():
+    rows, cols = inputs.bipartite_edges(40, 30, 500, 3)
+    rowptr, cidx = _csr(rows, cols, 40, 30)
+    rs = np.random.RandomState(1)
+    users, negs = rs.randint(0, 40, size=23), rs.randint(0, 30, size=23)
+    seed = 0xDEADBEEF12345678
+    got = D.neg_candidates(users, negs, 7, rowptr, cidx, 30, seed)
+    assert got.shape == (23, 7) and np.array_equal(got[:, 0], negs)
+    for b in range(23):
+        for j in range(1, 7):
+            assert got[b, j] == _scalar_candidate(users[b], b, j, rowptr, cidx, 30, seed), (b, j)
+    assert not np.array_equal(got, D.neg_candidates(users, negs, 7, rowptr, cidx, 30, seed + 1))
+
+
+def test_candidate_cap_and_a_user_with_one_free_item():
+    n_item = 6
+    # user 0 has every item (the draw is capped: the last of 256 draws), user 1 every item but 4
+    rows = np.array([0] * n_item + [1] * (n_item - 1))
+    cols = np.array(list(range(n_item)) + [0, 1, 2, 3, 5])
+    rowptr, cidx = _csr(rows, cols, 2, n_item)
+    got = D.neg_candidates([0, 1, 0, 1], [5, 4, 2, 4], 9, rowptr, cidx, n_item, 99)
+    for b in (0, 2):
+        for j in range(1, 9):
+            last = int(P.philox4x32_10(b, j, 63, D.TAG_DNSC, 99)[3])
+            assert got[b, j] == (last * n_item) >> 32
+    assert (got[[1, 3], 1:] == 4).all()
+
+
+def test_oracle_selection_ties_and_nan():
+    u = torch.tensor([[1.0, 0.0]])
+    items = torch.tensor([[0.5, 0.0], [2.0, 1.0], [2.0, -1.0], [float('nan'), 0.0], [-1.0, 0.0]])
+    ancs = torch.tensor([0, 0, 0])
+    cands = torch.tensor([[0, 1, 2], [3, 2, 1], [3, 3, 3]])
+    assert D.hard_negatives(u, items, ancs, cands).tolist() == [1, 2, 3]       # tie to the lowest j; NaN skipped; all NaN -> j = 0
+
+
+@pytest.mark.parametrize('value', [0, 257, -3, 2.5, True, '8', None])
+def test_bad_values_are_refused_at_construction(value):
+    with pytest.raises(ValueError, match='dns_candidates'):
+        make_run('lightgcn', train=dict(dns_candidates=value))
+
+
+@pytest.mark.parametrize('key', ['lightgcn', 'simgcl', 'sgl', 'ncl', 'hccf', 'lightgcl'])
+def test_every_bpr_model_accepts_the_key(key):
+    m, _, _ = make_run(key, train=dict(dns_candidates=256))
+    assert m.dns_candidates == 256 and m.dns_negs is None
+    assert make_run(key)[0].dns_candidates == 1
+
+
+def test_directau_is_refused():
+    assert make_run('directau', train=dict(dns_candidates=1))[0].dns_candidates == 1
+    with pytest.raises(ValueError, match='DirectAU trains without negatives'):
+        make_run('directau', train=dict(dns_candidates=2))
+
+
+def test_multi_gpu_is_refused():
+    from sslrec_b200.trainer import Trainer
+    m, _, dh = make_run('simgcl', train=dict(dns_candidates=8))
+    with pytest.raises(ValueError, match='single-GPU'):
+        m.shard_to(types.SimpleNamespace(shard_propagation=False))
+    assert m.comm is None
+    with pytest.raises(ValueError, match='single-GPU'):
+        Trainer(dh, grad_sync=object())
+    m, _, dh = make_run('simgcl')
+    Trainer(dh, grad_sync=object())             # without the key nothing changes
+
+
+def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
+    plain, dns = str(tmp_path / 'plain.pth'), str(tmp_path / 'dns.pth')
+    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
+    assert tr._resume_record(m, 'host')['dns_candidates'] == 8
+    tr.save_checkpoint(m, dns)
+    m, tr, _ = make_run('ncl', train=dict(dns_candidates=1))
+    assert 'dns_candidates' not in tr._resume_record(m, 'host')
+    tr.save_checkpoint(m, plain)
+    with pytest.raises(ValueError, match='dns_candidates: saved 8, now None'):
+        tr.load_checkpoint(m, dns)
+    m, tr, _ = make_run('ncl', train=dict(dns_candidates=4))
+    with pytest.raises(ValueError, match='dns_candidates: saved None, now 4'):
+        tr.load_checkpoint(m, plain)
+    with pytest.raises(ValueError, match='dns_candidates: saved 8, now 4'):
+        tr.load_checkpoint(m, dns)
+    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
+    assert tr.load_checkpoint(m, dns) == 0
