@@ -504,6 +504,38 @@ SSL_API int ssl_neg_candidates(const int64_t *users, const int64_t *negs, int64_
 SSL_API int ssl_neg_select(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
                            const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, int64_t *negs_out, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * a25  (no counterpart: MixGCF negatives, Huang et al. KDD 2021, optional key train.mixgcf)
+ *   ssl_mixgcf_bpr_fwd, for every pair b with u = U[ancs[b]], pbar = I[poss[b]] (rows of the summed
+ *   table the BPR term reads), X_l the item rows of layer l = 0 .. n_layers-1 (layer 0 = E0) and
+ *   candidates c_j = cands[b, j], j < M:
+ *     alpha_l = u01(Philox4x32-10(ctr (b, l, 0, "MIXA"), key seed_key(seed)).x), or alpha_in[b, l]
+ *     m_jl[k] = fmaf(alpha_l, X_l[p][k], (1 - alpha_l) * X_l[c_j][k])          (1 - alpha_l in fp32)
+ *     s_jl    = one sequential fp32 FMA chain over k of u[k] * m_jl[k]
+ *     j*_l    = argmax_j s_jl: lowest j on ties, NaN never wins, all NaN -> 0 (ssl_neg_select's rule)
+ *     nhat    = ((m_{j*_0,0} + m_{j*_1,1}) + m_{j*_2,2}) + ...                  (sum pooling, layer order)
+ *     z       = chain(u . nhat) - chain(u . pbar);  loss_b = softplus(z) (threshold-20 tail),
+ *     coef_b  = sigmoid(z);  picks[b, l] = c_{j*_l};  alpha_out[b, l] = alpha_l;  nhat [n_pairs, dim].
+ *   The seed is *seed_ptr when seed_ptr is non-null (CUDA-graph replay), else seed.  layer_tbls /
+ *   layer_strides are HOST arrays of n_layers entries (item 0's row, row stride in elements).
+ *   ssl_mixgcf_bpr_bwd, g = scale * (*gscale) * coef_b[b], gu = g * u (atomicAdd):
+ *     g_users[ancs[b]] += g (nhat - pbar);   g_items[poss[b]] += -gu;
+ *     g_layers[l][poss[b]] += alpha_l gu;    g_layers[l][picks[b, l]] += (1 - alpha_l) gu
+ *   (g_layers / gl_strides host arrays).  Identity ids into -0.0 stages give the per-position
+ *   contributions train.deterministic scatters in order; the numbering is in csrc/mixgcf.cuh.
+ *   1 <= M <= 256, 1 <= n_layers <= 8, dim <= SSL_MAX_DIM; n_pairs = 0 is a no-op for both.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_mixgcf_bpr_fwd(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride,
+                               const float *const *layer_tbls, const int64_t *layer_strides, int32_t n_layers, const int64_t *ancs,
+                               const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, uint64_t seed,
+                               const uint64_t *seed_ptr, const float *alpha_in, float *loss_b, float *coef_b, int64_t *picks,
+                               float *alpha_out, float *nhat, void *stream);
+SSL_API int ssl_mixgcf_bpr_bwd(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
+                               const int64_t *poss, const int64_t *picks, int64_t n_pairs, int32_t n_layers, int32_t dim,
+                               const float *nhat, const float *alpha, const float *coef_b, const float *gscale, float scale,
+                               float *g_users, int64_t gu_stride, float *g_items, int64_t gi_stride, float *const *g_layers,
+                               const int64_t *gl_strides, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -111,6 +111,10 @@ def _load():
         'ssl_scatter_rows_ordered': (C.c_int, [vp, vp, vp, i64, i32, vp, i64, vp]),
         'ssl_neg_candidates': (C.c_int, [vp, vp, i64, i32, vp, vp, i64, C.c_uint64, vp, vp, vp]),
         'ssl_neg_select': (C.c_int, [vp, i64, vp, i64, vp, vp, i64, i32, i32, vp, vp]),
+        'ssl_mixgcf_bpr_fwd': (C.c_int, [vp, i64, vp, i64, C.POINTER(vp), c_i64p, i32, vp, vp, vp, i64, i32, i32, C.c_uint64, vp, vp,
+                                         vp, vp, vp, vp, vp, vp]),
+        'ssl_mixgcf_bpr_bwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, f32, vp, i64, vp, i64,
+                                         C.POINTER(vp), c_i64p, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export what the header declares

@@ -90,18 +90,53 @@ class BaseModel(nn.Module):
         self.dns_negs = None
         if self.dns_candidates > 1 and not self.bpr_negatives:
             raise ValueError(f'train.dns_candidates: {type(self).__name__} trains without negatives')
+        # optional key train.mixgcf (MixGCF, with the M candidates of train.dns_candidates): the BPR term's negative is mixed
+        # from the positive and the candidates layer by layer; ``mixgcf_picks`` / ``mixgcf_alpha`` ([B, L+1]) keep the last
+        # step's picked items and mixing weights
+        self.mixgcf = E.mixgcf()
+        self.mixgcf_picks = self.mixgcf_alpha = None
+        self._mix_seed = None
+        self._mix_alpha_in = None      # tests: injected [B, L+1] mixing weights instead of the seeded draw
+        if self.mixgcf and not self.bpr_negatives:
+            raise ValueError(f'train.mixgcf: {type(self).__name__} trains without negatives')
+        if self.mixgcf and getattr(self, 'layer_num', 0) + 1 > E.MIXGCF_MAX_LAYERS:
+            raise ValueError(f'train.mixgcf mixes at most {E.MIXGCF_MAX_LAYERS} layers (layer_num + 1), got {self.layer_num + 1}')
 
-    bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates applies)
+    bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / train.mixgcf apply)
 
     def _dns_candidates(self, ancs, negs):
         """The batch's [B, M] DNS candidates (``engine.neg_candidates``; column 0 = the loader's ``negs``), or None when
-        train.dns_candidates is 1.  Their seed is the last one the step draws, so a DNS step draws every seed of the plain
-        step in the same order."""
-        if self.dns_candidates == 1:
+        train.dns_candidates is 1 and train.mixgcf is off.  Their seed is the last one the step draws, so a DNS step draws every
+        seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed, and with M = 1 its candidates
+        are the loader's negatives (no draw)."""
+        if self.dns_candidates == 1 and not self.mixgcf:
             return None
         from . import engine as E
+        seed = self._seeds.next()
+        self._mix_seed = seed
+        if self.dns_candidates == 1:
+            return E._i64(negs, ancs.device).view(-1, 1)
         rowptr, cols = self._train_csr(ancs.device)
-        return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, self._seeds.next())
+        return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed)
+
+    def _bpr_term(self, users, items, item_layers, ancs, poss, negs, cands, bpr):
+        """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term; with DNS the term on
+        the selected candidates (which the other terms then read too); with MixGCF ``engine.mixgcf_bpr_sum`` on the candidates
+        (the other terms keep the loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors;
+        ``item_layers()`` lists the item rows of its layers 0 .. L (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the
+        plain and DNS terms call (a model passes its module's, so a restatement can stand in for it)."""
+        from . import engine as E
+        if self.mixgcf:
+            loss, self.mixgcf_picks, self.mixgcf_alpha = E.mixgcf_bpr_sum(users, items, item_layers(), ancs, poss, cands, self._mix_seed,
+                                                                          self._mix_alpha_in)
+            return loss, negs
+        rows = isinstance(users, E.Rows)
+        if cands is not None:
+            negs = self._dns_select(users if rows else users.detach(), items if rows else items.detach(), ancs, cands)
+        if rows:
+            return bpr(users, items, ancs, poss, negs), negs
+        at = E.rows_at          # table[ids]; under train.deterministic with an ordered backward
+        return bpr(at(users, ancs), at(items, poss), at(items, negs)), negs
 
     def _dns_select(self, users, items, ancs, cands) -> torch.Tensor:
         """The highest-scored candidate of every pair on the rows the BPR term reads (``engine.hard_negatives``), kept as ``dns_negs``."""
@@ -140,6 +175,8 @@ class BaseModel(nn.Module):
             raise RuntimeError('train.deterministic is single-GPU: a row-sharded model sums its partials across GPUs in an order of its own')
         if comm is not None and self.dns_candidates > 1:
             raise ValueError('train.dns_candidates is single-GPU: a row-sharded model does not select hard negatives')
+        if comm is not None and self.mixgcf:
+            raise ValueError('train.mixgcf is single-GPU: a row-sharded model does not mix negatives')
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

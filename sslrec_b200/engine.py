@@ -1505,6 +1505,162 @@ def hard_negatives(users, items, ancs, cands: torch.Tensor) -> torch.Tensor:
     return out
 
 
+# ---- MixGCF negatives (optional key train.mixgcf) ----------------------------------------------------------------------------
+
+MIXGCF_MAX_LAYERS = 8
+
+
+def mixgcf() -> bool:
+    """The optional key ``train.mixgcf`` (INTEGRATION §2): True replaces the BPR term's negative by MixGCF's mixed negative
+    (``mixgcf_bpr_sum``); False (the default) is the plain step.  Raises ValueError for a value that is not a bool."""
+    from .config import configs
+    on = configs.get('train', {}).get('mixgcf', False)
+    if not isinstance(on, bool):
+        raise ValueError(f'train.mixgcf must be true or false, got {on!r}')
+    return on
+
+
+def _mix_grad_target(op, plain_grads: dict):
+    """Where an operand's gradient goes: a Rows' sink, or the zeroed gradient of a plain tensor (one per distinct tensor)."""
+    if isinstance(op, Rows):
+        return op.grad_ptr(), op.grad_stride
+    k, t = op
+    if k not in plain_grads:
+        plain_grads[k] = torch.zeros(t.shape, device=t.device, dtype=torch.float32)
+    return plain_grads[k].data_ptr(), t.shape[1]
+
+
+def _mix_table(op):
+    return _score_table(op if isinstance(op, Rows) else op[1])
+
+
+def _scatter_grouped(parts) -> None:
+    """Ordered scatter of (stage, ids, sink pointer, sink stride) parts.  Parts that address the same sink (pointer and stride) are
+    ONE scatter over their concatenated positions, in part order; the groups run in the order of their first part."""
+    groups: Dict[tuple, list] = {}
+    for stage, ids, ptr, stride in parts:
+        groups.setdefault((ptr, stride), []).append((stage, ids))
+    for (ptr, stride), ps in groups.items():
+        if len(ps) == 1:
+            scatter_rows_ordered(ps[0][0], ps[0][1], ptr, stride)
+        else:
+            scatter_rows_ordered(torch.cat([s for s, _ in ps]), torch.cat([i for _, i in ps]), ptr, stride)
+
+
+class _MixgcfFn(torch.autograd.Function):
+    """MixGCF's BPR term (``ssl_mixgcf_bpr_fwd`` / ``_bwd``).  Operands are Rows (gradients into their sinks, autograd sees their
+    tokens) or (index, tensor) of the plain tensors passed after ``pack`` (gradients into zeroed tensors returned to autograd)."""
+
+    @staticmethod
+    def forward(ctx, pack, *inputs):
+        ops, ancs, poss, cands, seed, alpha_in, n_plain = pack
+        users, items, layers = ops[0], ops[1], ops[2:]
+        u_ptr, u_stride, d = _mix_table(users)
+        i_ptr, i_stride, d_i = _mix_table(items)
+        tabs = [_mix_table(op) for op in layers]
+        if d_i != d or any(t[2] != d for t in tabs):
+            raise RuntimeError('sslrec_b200: the user, item and layer rows of a MixGCF term differ in width')
+        dev = cands.device
+        B, m = cands.shape
+        L1 = len(layers)
+        f = dict(device=dev, dtype=torch.float32)
+        loss_b, coef, out = torch.empty(B, **f), torch.empty(B, **f), torch.empty((), **f)
+        picks = torch.empty(B, L1, dtype=torch.int64, device=dev)
+        alpha, nhat = torch.empty(B, L1, **f), torch.empty(B, d, **f)
+        lp = (C.c_void_p * L1)(*[t[0] for t in tabs])
+        ls = (C.c_int64 * L1)(*[t[1] for t in tabs])
+        with torch.cuda.device(dev), _timed('mixgcf_fwd', dict(B=B, M=m, layers=L1, dim=d)):
+            s = _stream(cands)
+            check(lib.ssl_mixgcf_bpr_fwd(u_ptr, u_stride, i_ptr, i_stride, lp, ls, L1, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(),
+                                         B, m, d, int(seed), getattr(seed, 'ptr', 0) or None, _ptr(alpha_in), loss_b.data_ptr(),
+                                         coef.data_ptr(), picks.data_ptr(), alpha.data_ptr(), nhat.data_ptr(), s), 'ssl_mixgcf_bpr_fwd')
+            check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0, out.data_ptr(), s), 'ssl_sum')
+        ctx.pack = (ops, ancs, poss, picks, alpha, nhat, coef, n_plain, len(inputs) - n_plain)
+        ctx.mark_non_differentiable(picks, alpha)
+        return out, picks, alpha
+
+    @staticmethod
+    def backward(ctx, g, _g_picks, _g_alpha):
+        ops, ancs, poss, picks, alpha, nhat, coef, n_plain, n_tokens = ctx.pack
+        g = g.contiguous()
+        users, items, layers = ops[0], ops[1], ops[2:]
+        B, L1 = picks.shape
+        d = nhat.shape[1]
+        plain_grads: dict = {}
+        targets = [_mix_grad_target(op, plain_grads) for op in ops]
+        if any(p is None for p, _ in targets):
+            raise RuntimeError('sslrec_b200: every operand of a MixGCF term must take a gradient')
+        (gu, gu_s), (gi, gi_s), gl = targets[0], targets[1], targets[2:]
+        dev = g.device
+        with torch.cuda.device(dev), _timed('mixgcf_bwd', dict(B=B, layers=L1, dim=d)):
+            s = _stream(g)
+            if deterministic():
+                # identity ids on gathered rows into -0.0 stages (positions: csrc/mixgcf.cuh), then the ordered scatters
+                ug = _gather_rows(users, ancs)
+                pg = _gather_rows(items, poss)
+                ar = torch.arange(B, device=dev)
+                ids = (ar + B).unsqueeze(1).expand(B, L1).contiguous()
+                stage = _stage((2 + 2 * L1) * B, d, dev)
+                su, si = stage[:B], stage[B:2 * B]
+                sl = [stage[(2 + 2 * l) * B:(4 + 2 * l) * B] for l in range(L1)]
+                lp = (C.c_void_p * L1)(*[t.data_ptr() for t in sl])
+                ls = (C.c_int64 * L1)(*([d] * L1))
+                check(lib.ssl_mixgcf_bpr_bwd(ug.data_ptr(), d, pg.data_ptr(), d, ar.data_ptr(), ar.data_ptr(), ids.data_ptr(), B, L1, d,
+                                             nhat.data_ptr(), alpha.data_ptr(), coef.data_ptr(), g.data_ptr(), 1.0, su.data_ptr(), d,
+                                             si.data_ptr(), d, lp, ls, s), 'ssl_mixgcf_bpr_bwd')
+                parts = [(su, ancs, gu, gu_s), (si, poss, gi, gi_s)]
+                parts += [(sl[l], torch.cat([poss, picks[:, l]]), p, st) for l, (p, st) in enumerate(gl)]
+                _scatter_grouped(parts)
+            else:
+                u_ptr, u_stride, _ = _mix_table(users)
+                i_ptr, i_stride, _ = _mix_table(items)
+                lp = (C.c_void_p * L1)(*[p for p, _ in gl])
+                ls = (C.c_int64 * L1)(*[st for _, st in gl])
+                check(lib.ssl_mixgcf_bpr_bwd(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), picks.data_ptr(), B, L1, d,
+                                             nhat.data_ptr(), alpha.data_ptr(), coef.data_ptr(), g.data_ptr(), 1.0, gu, gu_s, gi, gi_s,
+                                             lp, ls, s), 'ssl_mixgcf_bpr_bwd')
+        zero = torch.zeros((), device=dev)
+        return (None,) + tuple(plain_grads[k] for k in range(n_plain)) + (zero,) * n_tokens
+
+
+def _gather_rows(op, ids: torch.Tensor) -> torch.Tensor:
+    """The rows ``ids`` of a MixGCF operand as a contiguous [len(ids), d] tensor."""
+    return op.take(ids) if isinstance(op, Rows) else op[1].index_select(0, ids)
+
+
+def mixgcf_bpr_sum(users, items, item_layers, ancs, poss, cands: torch.Tensor, seed, alpha=None):
+    """MixGCF's BPR term summed over the batch (``ssl_mixgcf_bpr_fwd``; formula in include/sslrec_b200.h, a25) -> (loss, picks
+    [B, L+1] int64, alpha [B, L+1] fp32).  ``users`` / ``items`` are the summed table the BPR term reads, ``item_layers`` the item
+    rows of its layers 0 .. L (layer 0 = E0), ``cands`` [B, M] the candidates (column 0 the loader's negative).  Each table is a
+    :class:`Rows` (gradient into its sink) or a [n, d] fp32 tensor (gradient through autograd, like ``rows_at``); under
+    ``deterministic()`` every batch row's gradient is added in position order.  The alpha draw is keyed by ``seed`` (a
+    :class:`DevSeed` passes its device word); ``alpha`` [B, L+1] fp32 injects the mixing weights instead."""
+    layers = list(item_layers)
+    if not 1 <= len(layers) <= MIXGCF_MAX_LAYERS:
+        raise ValueError(f'MixGCF mixes 1 .. {MIXGCF_MAX_LAYERS} layers, got {len(layers)}')
+    dev = cands.device
+    ancs, poss, cands = _i64(ancs, dev), _i64(poss, dev), _i64(cands, dev)
+    if cands.dim() != 2 or ancs.numel() != cands.shape[0] or poss.numel() != cands.shape[0]:
+        raise RuntimeError('sslrec_b200: one anchor, one positive and one row of candidates per pair')
+    if alpha is not None:
+        alpha = alpha.to(device=dev, dtype=torch.float32).contiguous()
+        if tuple(alpha.shape) != (cands.shape[0], len(layers)):
+            raise RuntimeError('sslrec_b200: injected alpha must be [B, L+1]')
+    plain: List[torch.Tensor] = []
+    ops = []
+    for t in [users, items] + layers:
+        if isinstance(t, Rows):
+            ops.append(t)
+            continue
+        k = next((i for i, q in enumerate(plain) if q is t), None)      # one gradient per distinct tensor
+        if k is None:
+            plain.append(t)
+            k = len(plain) - 1
+        ops.append((k, t.detach()))
+    pack = (ops, ancs, poss, cands, seed, alpha, len(plain))
+    return _MixgcfFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
+
+
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------
 
 def _rowgemm(in1, k1, m1, m1_trans, out, n_out, scale=1.0, slope=1.0, accumulate=False, in2=None, k2=0, m2=None, m2_trans=False, pre_ref=None,

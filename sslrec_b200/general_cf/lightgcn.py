@@ -40,6 +40,14 @@ class LightGCN(BaseModel):
         self._state = st
         return st
 
+    def _mix_keep(self):
+        """Layers the propagation keeps for train.mixgcf: 1 .. L (their item rows are mixed); none without the key."""
+        return tuple(range(1, self.layer_num + 1)) if self.mixgcf else ()
+
+    def _mix_layers(self, st, v):
+        """The item rows of layers 0 .. L of view ``v`` (layer 0 = E0), for ``_bpr_term``."""
+        return lambda: [st.items(v, k) for k in range(self.layer_num + 1)]
+
     def _edge_view(self, keep_rate, slot=0):
         inj = None if self._inject is None else self._inject.get('edge_masks', [None] * 4)[slot]
         return self.edge_dropper.view(keep_rate, self._seeds.next(), injected=inj)
@@ -56,12 +64,10 @@ class LightGCN(BaseModel):
     def cal_loss(self, batch_data):
         self.is_training = True
         ancs, poss, negs = batch_data
-        st = self._propagate([self._edge_view(self.keep_rate)])
+        st = self._propagate([self._edge_view(self.keep_rate)], keep_layers=self._mix_keep())
         self.final_embeds = st.E.view(st.n, st.dim)
         cands = self._dns_candidates(ancs, negs)
-        if cands is not None:
-            negs = self._dns_select(st.users(0), st.items(0), ancs, cands)
-        bpr_loss = cal_bpr_loss(st.users(0), st.items(0), ancs, poss, negs) / ancs.shape[0]
+        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
         reg_loss = self.reg_weight * reg_params(self)
         loss = bpr_loss + reg_loss
         losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss}

@@ -64,7 +64,7 @@ class NCL(LightGCN):
     def _run(self):
         ctx_layer = self.high_order * 2
         iteration = max(self.layer_num, ctx_layer)                                              # ncl.py:36
-        return self._propagate([E.ViewSpec()], n_layers=iteration, sum_layers=self.layer_num, keep_layers=(ctx_layer,))
+        return self._propagate([E.ViewSpec()], n_layers=iteration, sum_layers=self.layer_num, keep_layers=(ctx_layer,) + self._mix_keep())
 
     def forward(self, adj):
         """-> (summed embeddings [N, d], state); ``state.all_nodes(0, k).dense()`` is layer k."""
@@ -83,8 +83,6 @@ class NCL(LightGCN):
             self._cluster()
         embeds, st = self.forward(self.adj)
         cands = self._dns_candidates(ancs, negs)
-        if cands is not None:
-            negs = self._dns_select(st.users(0), st.items(0), ancs, cands)
         ctx = self.high_order * 2
         bsz = ancs.shape[0]
         # structure loss (ncl.py:51-58): context (layer 2*high_order) vs ego (layer 0), all ego rows as negatives
@@ -96,7 +94,7 @@ class NCL(LightGCN):
                       + cal_infonce_loss(st.items(0, 0), ic, ic, self.temperature, idx=poss, idx2=self.item2cluster[poss])) / bsz
         struct_loss = struct_loss * self.struct_weight
         proto_loss = proto_loss * self.proto_weight
-        bpr_loss = cal_bpr_loss(st.users(0), st.items(0), ancs, poss, negs) / bsz
+        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / bsz
         reg_loss = reg_params(self) * self.reg_weight
         loss = bpr_loss + struct_loss + proto_loss + reg_loss
         losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'struct_loss': struct_loss, 'proto_loss': proto_loss}

@@ -47,12 +47,12 @@ class SGL(LightGCN):
         cands = self._dns_candidates(ancs, negs)
         rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
         v0.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
-        st = self._propagate([v0, v1, E.ViewSpec()], n_layers=configs['model']['layer_num'])
+        st = self._propagate([v0, v1, E.ViewSpec()], n_layers=configs['model']['layer_num'], keep_layers=self._mix_keep())
         self.final_embeds = st.E[:, 2, :]
-        if cands is not None:
-            negs = self._dns_select(st.users(2), st.items(2), ancs, cands)
         bsz = ancs.shape[0]
-        bpr_loss = cal_bpr_loss(st.users(2), st.items(2), ancs, poss, negs) / bsz
+        # with train.mixgcf the idx=negs term below keeps the loader's negatives
+        bpr_loss, negs = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, cands, cal_bpr_loss)
+        bpr_loss = bpr_loss / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \
             cal_infonce_loss(st.items(0), st.items(1), st.items(1), self.temperature, idx=poss) + \
             cal_infonce_loss(st.items(0), st.items(1), st.items(1), self.temperature, idx=negs)

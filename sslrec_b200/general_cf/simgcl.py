@@ -38,11 +38,9 @@ class SimGCL(LightGCN):
         cands = self._dns_candidates(ancs, negs)
         rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
         v0.row_bits = v2.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
-        st = self._propagate([v0, v1, v2], noise_eps=self.eps)
-        if cands is not None:
-            negs = self._dns_select(st.users(2), st.items(2), ancs, cands)
+        st = self._propagate([v0, v1, v2], noise_eps=self.eps, keep_layers=self._mix_keep())
         bsz = ancs.shape[0]
-        bpr_loss = cal_bpr_loss(st.users(2), st.items(2), ancs, poss, negs) / bsz
+        bpr_loss = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, cands, cal_bpr_loss)[0] / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \
             cal_infonce_loss(st.items(0), st.items(1), st.items(1), self.temperature, idx=poss)
         cl_loss = cl_loss / bsz

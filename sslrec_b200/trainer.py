@@ -105,6 +105,8 @@ class Trainer(object):
         self.grad_sync = grad_sync     # parallel.BatchShard: data-parallel ranks average gradients before the step
         if grad_sync is not None and E.dns_candidates() > 1:
             raise ValueError('train.dns_candidates is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
+        if grad_sync is not None and E.mixgcf():
+            raise ValueError('train.mixgcf is single-GPU: data-parallel ranks share the seed, so their mixing weights would coincide')
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
         self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
@@ -318,6 +320,8 @@ class Trainer(object):
                   'batch_size': t['batch_size'], 'seed': t.get('seed'), 'loader': kind, 'deterministic': E.deterministic()}
         if E.dns_candidates() > 1:          # only then: the records of runs without the key stay as they were
             record['dns_candidates'] = E.dns_candidates()
+        if E.mixgcf():
+            record['mixgcf'] = True
         return record
 
     def save_checkpoint(self, model, path):
