@@ -536,6 +536,36 @@ SSL_API int ssl_mixgcf_bpr_bwd(const float *u_tbl, int64_t u_stride, const float
                                float *g_users, int64_t gu_stride, float *g_items, int64_t gi_stride, float *const *g_layers,
                                const int64_t *gl_strides, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * a26  (no counterpart: sampled softmax loss, Wu et al. TOIS 2023, optional key
+ *   train.ssm_temperature = tau; the reference's data handler leaves room for a non-pairwise
+ *   loss, data_handler_general_cf.py:84-88)
+ *   ssl_ssm_fwd, for every pair b with u = U[ancs[b]], c_0 = I[poss[b]], c_q = I[cands[b, q-1]]
+ *   (q = 1 .. M; column q of every [n_pairs, M+1] array), x^ = x / sqrt(1e-8 + |x|^2) as in the
+ *   InfoNCE terms (loss_utils.py:30-39):
+ *     s_q    = (u^ . c^_q) / tau;   loss_b = lse_q(s_q) - s_0 (max-shifted, fp32; a NaN score makes
+ *              loss_b NaN);   w_q = softmax(s)_q - [q = 0];   nrm[b] = (n_u, n_0 .. n_M)
+ *   in the fp32 order of csrc/ssm.cuh: per float4 slot a 4-term FMA chain, the slots summed by a
+ *   fixed xor-butterfly tree, s_q = dot / ((n_u * n_q) * tau), the exp sum per lane over
+ *   q = t (mod G) then the same tree.  Outputs loss_b [n_pairs], s, w [n_pairs, M+1], nrm [n_pairs, M+2].
+ *   ssl_ssm_bwd, g = scale * (*gscale) (gscale may be NULL), with float atomics:
+ *     g_items[c_q] += g w_q (u^ / tau - s_q c^_q) / n_q        (each q as it comes)
+ *     g_users[ancs[b]] += g sum_q w_q (c^_q / tau - s_q u^) / n_u  (summed in q order, added once)
+ *   Duplicate candidates are separate terms adding into one row (no de-duplication, no logQ
+ *   correction: the sampler is uniform).  Identity ids into -0.0 stages give the per-position
+ *   contributions train.deterministic scatters in order; the numbering is in csrc/ssm.cuh.
+ *   1 <= M <= 256; dim a multiple of 4, <= SSL_MAX_DIM; tau finite and > 0; every table and sink
+ *   16-byte aligned with a stride (elements) that is a multiple of 4 and >= dim.  n_pairs = 0 is
+ *   a no-op for both; rejected arguments write nothing.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_ssm_fwd(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
+                        const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, float tau, float *loss_b,
+                        float *s, float *w, float *nrm, void *stream);
+SSL_API int ssl_ssm_bwd(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
+                        const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, float tau, const float *s,
+                        const float *w, const float *nrm, const float *gscale, float scale, float *g_users, int64_t gu_stride,
+                        float *g_items, int64_t gi_stride, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

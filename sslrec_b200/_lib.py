@@ -115,6 +115,8 @@ def _load():
                                          vp, vp, vp, vp, vp, vp]),
         'ssl_mixgcf_bpr_bwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, f32, vp, i64, vp, i64,
                                          C.POINTER(vp), c_i64p, vp]),
+        'ssl_ssm_fwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp]),
+        'ssl_ssm_bwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, f32, vp, i64, vp, i64, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export what the header declares

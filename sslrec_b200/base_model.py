@@ -101,17 +101,30 @@ class BaseModel(nn.Module):
             raise ValueError(f'train.mixgcf: {type(self).__name__} trains without negatives')
         if self.mixgcf and getattr(self, 'layer_num', 0) + 1 > E.MIXGCF_MAX_LAYERS:
             raise ValueError(f'train.mixgcf mixes at most {E.MIXGCF_MAX_LAYERS} layers (layer_num + 1), got {self.layer_num + 1}')
+        # optional key train.ssm_temperature = tau (sampled softmax loss, with the M candidates of train.dns_candidates): the BPR
+        # term is replaced by a softmax of the positive against the candidates on cosine scores over tau, reported as ssm_loss
+        self.ssm_temperature = E.ssm_temperature()
+        if self.ssm_temperature is not None and not self.bpr_negatives:
+            raise ValueError(f'train.ssm_temperature: {type(self).__name__} trains without negatives')
+        if self.ssm_temperature is not None and self.mixgcf:
+            raise ValueError('train.ssm_temperature and train.mixgcf both replace the BPR term: set one of them')
 
-    bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / train.mixgcf apply)
+    bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / mixgcf / ssm_temperature apply)
+
+    @property
+    def bpr_loss_name(self) -> str:
+        """The name ``cal_loss`` reports the BPR term under: 'ssm_loss' when train.ssm_temperature replaces it, else 'bpr_loss'."""
+        return 'bpr_loss' if self.ssm_temperature is None else 'ssm_loss'
 
     def _dns_candidates(self, ancs, negs):
         """The batch's [B, M] DNS candidates (``engine.neg_candidates``; column 0 = the loader's ``negs``), or None when
-        train.dns_candidates is 1 and train.mixgcf is off.  Their seed is the last one the step draws, so a DNS step draws every
-        seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed, and with M = 1 its candidates
-        are the loader's negatives (no draw)."""
-        if self.dns_candidates == 1 and not self.mixgcf:
-            return None
+        train.dns_candidates is 1 and neither train.mixgcf nor train.ssm_temperature is set.  Their seed is the last one the step
+        draws, so a DNS step draws every seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed,
+        and with M = 1 its candidates are the loader's negatives (no draw).  The sampled softmax loss with M = 1 takes the
+        loader's negatives without drawing a seed."""
         from . import engine as E
+        if self.dns_candidates == 1 and not self.mixgcf:
+            return None if self.ssm_temperature is None else E._i64(negs, ancs.device).view(-1, 1)
         seed = self._seeds.next()
         self._mix_seed = seed
         if self.dns_candidates == 1:
@@ -121,8 +134,8 @@ class BaseModel(nn.Module):
 
     def _bpr_term(self, users, items, item_layers, ancs, poss, negs, cands, bpr):
         """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term; with DNS the term on
-        the selected candidates (which the other terms then read too); with MixGCF ``engine.mixgcf_bpr_sum`` on the candidates
-        (the other terms keep the loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors;
+        the selected candidates (which the other terms then read too); with MixGCF ``engine.mixgcf_bpr_sum`` and with
+        train.ssm_temperature ``engine.ssm_loss_sum`` on the candidates (the other terms keep the loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors;
         ``item_layers()`` lists the item rows of its layers 0 .. L (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the
         plain and DNS terms call (a model passes its module's, so a restatement can stand in for it)."""
         from . import engine as E
@@ -130,6 +143,8 @@ class BaseModel(nn.Module):
             loss, self.mixgcf_picks, self.mixgcf_alpha = E.mixgcf_bpr_sum(users, items, item_layers(), ancs, poss, cands, self._mix_seed,
                                                                           self._mix_alpha_in)
             return loss, negs
+        if self.ssm_temperature is not None:
+            return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature), negs
         rows = isinstance(users, E.Rows)
         if cands is not None:
             negs = self._dns_select(users if rows else users.detach(), items if rows else items.detach(), ancs, cands)
@@ -177,6 +192,8 @@ class BaseModel(nn.Module):
             raise ValueError('train.dns_candidates is single-GPU: a row-sharded model does not select hard negatives')
         if comm is not None and self.mixgcf:
             raise ValueError('train.mixgcf is single-GPU: a row-sharded model does not mix negatives')
+        if comm is not None and self.ssm_temperature is not None:
+            raise ValueError('train.ssm_temperature is single-GPU: a row-sharded model does not score sampled candidates')
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

@@ -1646,19 +1646,117 @@ def mixgcf_bpr_sum(users, items, item_layers, ancs, poss, cands: torch.Tensor, s
         alpha = alpha.to(device=dev, dtype=torch.float32).contiguous()
         if tuple(alpha.shape) != (cands.shape[0], len(layers)):
             raise RuntimeError('sslrec_b200: injected alpha must be [B, L+1]')
+    ops, plain = _mix_operands([users, items] + layers)
+    pack = (ops, ancs, poss, cands, seed, alpha, len(plain))
+    return _MixgcfFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
+
+
+def _mix_operands(tables):
+    """-> (ops, plain): each table as an operand of ``_MixgcfFn`` / ``_SsmFn`` -- a Rows as it is, a plain tensor as (index,
+    detached tensor) into ``plain``, the distinct plain tensors (one gradient per distinct tensor)."""
     plain: List[torch.Tensor] = []
     ops = []
-    for t in [users, items] + layers:
+    for t in tables:
         if isinstance(t, Rows):
             ops.append(t)
             continue
-        k = next((i for i, q in enumerate(plain) if q is t), None)      # one gradient per distinct tensor
+        k = next((i for i, q in enumerate(plain) if q is t), None)
         if k is None:
             plain.append(t)
             k = len(plain) - 1
         ops.append((k, t.detach()))
-    pack = (ops, ancs, poss, cands, seed, alpha, len(plain))
-    return _MixgcfFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
+    return ops, plain
+
+
+# ---- sampled softmax loss (optional key train.ssm_temperature) ---------------------------------------------------------------
+
+def ssm_temperature() -> Optional[float]:
+    """The optional key ``train.ssm_temperature`` (INTEGRATION §2): tau, a finite number > 0 (int or float, not a bool), replaces
+    the BPR term by the sampled softmax loss on cosine scores over tau (``ssm_loss_sum``); absent or null (the default) is the
+    plain step.  Raises ValueError for any other value, or one that is not finite and > 0 in fp32."""
+    from .config import configs
+    t = configs.get('train', {}).get('ssm_temperature')
+    if t is None:
+        return None
+    if isinstance(t, bool) or not isinstance(t, (int, float)) or not (0.0 < C.c_float(t).value < math.inf):
+        raise ValueError(f'train.ssm_temperature must be a finite number > 0 or null, got {t!r}')
+    return float(t)
+
+
+class _SsmFn(torch.autograd.Function):
+    """The sampled softmax term (``ssl_ssm_fwd`` / ``_bwd``).  Operands as in ``_MixgcfFn``: Rows (gradients into their sinks,
+    autograd sees their tokens) or (index, tensor) of the plain tensors passed after ``pack``."""
+
+    @staticmethod
+    def forward(ctx, pack, *inputs):
+        ops, ancs, poss, cands, tau, n_plain = pack
+        users, items = ops
+        u_ptr, u_stride, d = _mix_table(users)
+        i_ptr, i_stride, d_i = _mix_table(items)
+        if d_i != d:
+            raise RuntimeError('sslrec_b200: the user and item rows of a sampled softmax term differ in width')
+        dev = cands.device
+        B, m = cands.shape
+        f = dict(device=dev, dtype=torch.float32)
+        loss_b, out = torch.empty(B, **f), torch.empty((), **f)
+        s, w, nrm = torch.empty(B, m + 1, **f), torch.empty(B, m + 1, **f), torch.empty(B, m + 2, **f)
+        with torch.cuda.device(dev), _timed('ssm_fwd', dict(B=B, M=m, dim=d)):
+            st = _stream(cands)
+            check(lib.ssl_ssm_fwd(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(), B, m, d, tau,
+                                  loss_b.data_ptr(), s.data_ptr(), w.data_ptr(), nrm.data_ptr(), st), 'ssl_ssm_fwd')
+            check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0, out.data_ptr(), st), 'ssl_sum')
+        ctx.pack = (ops, ancs, poss, cands, tau, s, w, nrm, n_plain, len(inputs) - n_plain)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        ops, ancs, poss, cands, tau, s, w, nrm, n_plain, n_tokens = ctx.pack
+        g = g.contiguous()
+        users, items = ops
+        B, m = cands.shape
+        d = _mix_table(users)[2]
+        plain_grads: dict = {}
+        targets = [_mix_grad_target(op, plain_grads) for op in ops]
+        if any(p is None for p, _ in targets):
+            raise RuntimeError('sslrec_b200: every operand of a sampled softmax term must take a gradient')
+        (gu, gu_s), (gi, gi_s) = targets
+        dev = g.device
+        with torch.cuda.device(dev), _timed('ssm_bwd', dict(B=B, M=m, dim=d)):
+            st = _stream(g)
+            if deterministic():
+                # identity ids on gathered rows into a -0.0 stage (positions: csrc/ssm.cuh), then the ordered scatters
+                item_ids = torch.cat([poss, cands.view(-1)])
+                ug, ig = _gather_rows(users, ancs), _gather_rows(items, item_ids)
+                ar = torch.arange(B, device=dev)
+                ci = torch.arange(B, B * (m + 1), device=dev)
+                stage = _stage(B * (m + 2), d, dev)
+                su, si = stage[:B], stage[B:]
+                check(lib.ssl_ssm_bwd(ug.data_ptr(), d, ig.data_ptr(), d, ar.data_ptr(), ar.data_ptr(), ci.data_ptr(), B, m, d, tau,
+                                      s.data_ptr(), w.data_ptr(), nrm.data_ptr(), g.data_ptr(), 1.0, su.data_ptr(), d, si.data_ptr(), d,
+                                      st), 'ssl_ssm_bwd')
+                _scatter_grouped([(su, ancs, gu, gu_s), (si, item_ids, gi, gi_s)])
+            else:
+                u_ptr, u_stride, _ = _mix_table(users)
+                i_ptr, i_stride, _ = _mix_table(items)
+                check(lib.ssl_ssm_bwd(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(), B, m, d, tau,
+                                      s.data_ptr(), w.data_ptr(), nrm.data_ptr(), g.data_ptr(), 1.0, gu, gu_s, gi, gi_s, st), 'ssl_ssm_bwd')
+        zero = torch.zeros((), device=dev)
+        return (None,) + tuple(plain_grads[k] for k in range(n_plain)) + (zero,) * n_tokens
+
+
+def ssm_loss_sum(users, items, ancs, poss, cands: torch.Tensor, temp: float) -> torch.Tensor:
+    """The sampled softmax loss summed over the batch (``ssl_ssm_fwd``; formula in include/sslrec_b200.h, a26): for every pair
+    lse_q(s_q) - s_0 over the positive (q = 0) and the candidates ``cands`` [B, M] (column 0 the loader's negative), with
+    s_q = cos(users[ancs[b]], items[c_q]) / temp.  ``users`` / ``items`` are each a :class:`Rows` (gradient into its sink; a
+    restricted view must mark every candidate row) or a [n, d] fp32 tensor (gradient through autograd, like ``rows_at``); under
+    ``deterministic()`` every batch row's gradient is added in position order."""
+    dev = cands.device
+    ancs, poss, cands = _i64(ancs, dev), _i64(poss, dev), _i64(cands, dev)
+    if cands.dim() != 2 or ancs.numel() != cands.shape[0] or poss.numel() != cands.shape[0]:
+        raise RuntimeError('sslrec_b200: one anchor, one positive and one row of candidates per pair')
+    ops, plain = _mix_operands([users, items])
+    pack = (ops, ancs, poss, cands, float(temp), len(plain))
+    return _SsmFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
 
 
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------

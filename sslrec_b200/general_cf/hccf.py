@@ -94,10 +94,11 @@ class HCCF(BaseModel):
         cands = self._dns_candidates(ancs, negs)
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (hccf.py:70-74)
         layers = lambda: [t[self.user_num:] for t in self._mix_tables]
-        terms = {'bpr_loss': self._bpr_term(users, items, layers, ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0],
+        bpr_loss = self._bpr_term(users, items, layers, ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
+        terms = {self.bpr_loss_name: bpr_loss,
                  'reg_loss': reg_params(self) * self.reg_weight,
                  'cl_loss': self._contrast(gcn_out, hyper_out, ancs, poss) * self.cl_weight}
-        return terms['bpr_loss'] + terms['reg_loss'] + terms['cl_loss'], terms
+        return bpr_loss + terms['reg_loss'] + terms['cl_loss'], terms
 
     def _eval_tables(self):
         embeds, _, _ = self.forward(self.adj, 1.0)

@@ -149,7 +149,7 @@ class LightGCL(BaseModel):
         reg_loss = reg_params(self) * self.reg_weight
         cl_loss = self.cl_weight * cl_loss
         loss = bpr_loss + cl_loss + reg_loss
-        losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
+        losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
         return loss, losses
 
     def _eval_tables(self):

@@ -70,7 +70,7 @@ class LightGCN(BaseModel):
         bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
         reg_loss = self.reg_weight * reg_params(self)
         loss = bpr_loss + reg_loss
-        losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss}
+        losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss}
         return loss, losses
 
     def _exact_forward(self):

@@ -97,7 +97,7 @@ class NCL(LightGCN):
         bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / bsz
         reg_loss = reg_params(self) * self.reg_weight
         loss = bpr_loss + struct_loss + proto_loss + reg_loss
-        losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'struct_loss': struct_loss, 'proto_loss': proto_loss}
+        losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss, 'struct_loss': struct_loss, 'proto_loss': proto_loss}
         return loss, losses
 
     def _eval_tables(self):

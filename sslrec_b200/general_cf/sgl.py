@@ -50,7 +50,7 @@ class SGL(LightGCN):
         st = self._propagate([v0, v1, E.ViewSpec()], n_layers=configs['model']['layer_num'], keep_layers=self._mix_keep())
         self.final_embeds = st.E[:, 2, :]
         bsz = ancs.shape[0]
-        # with train.mixgcf the idx=negs term below keeps the loader's negatives
+        # with train.mixgcf or train.ssm_temperature the idx=negs term below keeps the loader's negatives
         bpr_loss, negs = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, cands, cal_bpr_loss)
         bpr_loss = bpr_loss / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \
@@ -60,5 +60,5 @@ class SGL(LightGCN):
         reg_loss = self.reg_weight * reg_params(self)
         cl_loss = cl_loss * self.cl_weight
         loss = bpr_loss + reg_loss + cl_loss
-        losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
+        losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
         return loss, losses

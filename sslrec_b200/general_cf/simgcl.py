@@ -47,7 +47,7 @@ class SimGCL(LightGCN):
         reg_loss = self.reg_weight * reg_params(self)
         cl_loss = cl_loss * self.cl_weight
         loss = bpr_loss + reg_loss + cl_loss
-        losses = {'bpr_loss': bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
+        losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss, 'cl_loss': cl_loss}
         return loss, losses
 
     def _eval_tables(self):

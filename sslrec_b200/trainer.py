@@ -107,6 +107,8 @@ class Trainer(object):
             raise ValueError('train.dns_candidates is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
         if grad_sync is not None and E.mixgcf():
             raise ValueError('train.mixgcf is single-GPU: data-parallel ranks share the seed, so their mixing weights would coincide')
+        if grad_sync is not None and E.ssm_temperature() is not None:
+            raise ValueError('train.ssm_temperature is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
         self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
@@ -322,6 +324,8 @@ class Trainer(object):
             record['dns_candidates'] = E.dns_candidates()
         if E.mixgcf():
             record['mixgcf'] = True
+        if E.ssm_temperature() is not None:
+            record['ssm_temperature'] = E.ssm_temperature()
         return record
 
     def save_checkpoint(self, model, path):
