@@ -3,6 +3,7 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
+import mixgcf_oracle
 from oracle import cf_oracle as O
 from oracle import inputs, replay
 
@@ -207,7 +208,8 @@ def path_errors(got, ref):
     for k, g in ref['grads'].items():
         assert got['grads'][k].shape == g.shape, (k, got['grads'][k].shape, g.shape)
         r['grad_' + k] = frac(got['grads'][k], g, GRAD_RTOL * np.abs(g) + GRAD_MAXTOL * np.abs(g).max())
-    r['preds'] = frac(got['preds'], ref['preds'], PRED_RTOL * np.maximum(1.0, np.abs(ref['preds'])))
+    if 'preds' in ref:
+        r['preds'] = frac(got['preds'], ref['preds'], PRED_RTOL * np.maximum(1.0, np.abs(ref['preds'])))
     return r
 
 
@@ -259,6 +261,133 @@ def kink_margin(model_key, case, hp, adj, dr, st):
             s = prod.sum(1)
             see(s.abs() - 5.0, prod.abs().sum(1))
     return best[0]
+
+
+# ---- whole steps with the BPR term replaced: MixGCF and the sampled softmax loss (tests/test_gpu_mixgcf.py, test_gpu_ssm.py,
+# tests/test_host_mixgcf.py, test_host_ssm.py) ----------------------------------------------------------------------------------
+
+# (model_key, hyper-parameters over the goldens') of every BPR model.  NCL's context layer 2 high_order lies beyond (3, 2),
+# inside (3, 1) and at the last (2, 1) of the L + 1 layers MixGCF mixes; HCCF's hyper branch at two widths with injected drops
+BPR_TERM_MODELS = [('lightgcn', {}), ('simgcl', {}), ('sgl', {}),
+                   ('ncl', dict(layer_num=3, high_order=2)), ('ncl', dict(layer_num=3, high_order=1)), ('ncl', dict(layer_num=2, high_order=1)),
+                   ('hccf', dict(hyper_num=128, keep_rate=0.5)), ('hccf', dict(hyper_num=16, keep_rate=0.5)),
+                   ('lightgcl', dict(dropout=0))]
+BPR_TERM_DIMS = (20, 64, 128)       # the FFMA contraction with idle propagation lanes, a tensor-core contraction, the widest row
+BPR_TERM_TAU, BPR_TERM_SMALL_TAU = 0.1, 0.02
+# cases whose default seed puts a kink input within KINK_MARGIN of its |term| sum: the first later seed that does not
+BPR_TERM_SEEDS = {('simgcl', 128, None): 43, ('hccf', 64, 128): 43, ('hccf', 128, 128): 42}     # (model_key, dim, hyper_num)
+PICK_GAP_RTOL = 1e-4                # a MixGCF pick is decided when its score beats the runner-up by this much of their |terms|
+
+
+def bpr_term_cases(ssm: bool):
+    """(model_key, hyper-parameter overrides, embedding_size, M, sampled-softmax tau or None) of every whole-step case: each
+    BPR model at each dim with M = 8, one row at M = 32 and, for the sampled softmax loss, one row at a small tau."""
+    tau = BPR_TERM_TAU if ssm else None
+    out = [(m, hp, d, 8, tau) for m, hp in BPR_TERM_MODELS for d in BPR_TERM_DIMS]
+    out.append(('lightgcl', dict(dropout=0), 64, 32, tau))
+    if ssm:
+        out.append(('ncl', dict(layer_num=3, high_order=1), 64, 8, BPR_TERM_SMALL_TAU))
+    return out
+
+
+def bpr_term_case_id(case):
+    m, hp, d, M, tau = case
+    return '-'.join([m] + [f'{k}{v}' for k, v in sorted(hp.items())] + [f'd{d}', f'M{M}'] + ([] if tau is None else [f'tau{tau}']))
+
+
+def bpr_term_setup(model_key, hp_over, dim):
+    """-> case, hp, adjacency, draws and injected state of one whole-step case on the graph of ``path_case``."""
+    case = path_case(dim, seed=BPR_TERM_SEEDS.get((model_key, dim, hp_over.get('hyper_num')), 41))
+    hp = dict(path_hp(model_key, dim), **hp_over)
+    adj = O.normalized_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
+    dr = replay.draws(model_key, case, hp, adj)
+    return case, hp, adj, dr, path_state(model_key, case, hp, adj, dr)
+
+
+def bpr_tables(model_key, case, hp, adj, dr, params):
+    """The tables the BPR term of ``replay.oracle_loss`` reads, in the dtype of ``params``: (summed user table, summed item
+    table, item rows of layers 0 .. L of the same view).  LightGCN: its edge-dropped view; SimGCL, SGL: the un-augmented view;
+    NCL: the first L + 1 of its max(L, 2 high_order) layers; HCCF: x_k = gcn_(k-1) + hyper_(k-1) with the injected edge and
+    hyper keeps; LightGCL: the per-layer Z on its own adjacency (dropout 0)."""
+    name = model_key.split('_')[0]
+    ue, ie = params['user_embeds'], params['item_embeds']
+    dt, nu, L = ue.dtype, case['n_user'], hp['layer_num']
+    e0 = torch.cat([ue, ie], 0)
+    if name == 'ncl':
+        e, xs = O.ncl_embeds_list(adj.torch_coo(dt), e0, L, hp['high_order'])
+        xs = xs[:L + 1]
+    elif name == 'hccf':
+        e, gcn, hyp = O.hccf_embeds(adj, ue, ie, params['user_hyper_embeds'], params['item_hyper_embeds'], L, hp['keep_rate'],
+                                    hp['mult'], hp['leaky'], dr['edge_keeps'], dr['hyper_keeps'])
+        xs = [e0] + [g + h for g, h in zip(gcn, hyp)]
+    else:
+        if name == 'lightgcn':
+            a_t = O.edge_dropped(adj, dr['edge_keep'], hp['keep_rate'], False, dt)
+        elif name == 'lightgcl':
+            assert hp['dropout'] == 0
+            a_t = O.lightgcl_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item']).torch_coo(dt)
+        else:                                   # SimGCL's clean view, SGL's keep_rate 1.0 view
+            a_t = adj.torch_coo(dt)
+        xs = [e0]
+        for _ in range(L):
+            xs.append(torch.sparse.mm(a_t, xs[-1]))
+        e = sum(xs)
+    return e[:nu], e[nu:], [x[nu:] for x in xs]
+
+
+def bpr_part(model_key, ue, ie, batch):
+    """The BPR term of ``replay.oracle_loss`` on summed tables, in the oracle's own expression for the model."""
+    ancs, poss, negs = batch
+    a, p, n = ue[ancs], ie[poss], ie[negs]
+    if model_key.split('_')[0] in ('hccf', 'lightgcl'):
+        return -((a * p).sum(-1) - (a * n).sum(-1)).sigmoid().log().mean()
+    return O.bpr_loss_sum(a, p, n) / ancs.shape[0]
+
+
+def bpr_term_oracle(model_key, case, hp, adj, dr, st, dtype, term, name):
+    """The whole step of the oracle in ``dtype`` with its BPR term replaced: ``replay.oracle_loss`` minus its bpr_loss plus
+    ``term(users, items, item_layers) / B`` on the tables of ``bpr_tables``, reported as ``name``; backward -> dict(loss,
+    parts, grads) of float64 numpy, every parameter's gradient.  Asserts first that the tables are the ones the loss read:
+    the BPR term on them equals the oracle's bit for bit."""
+    params = path_params(model_key, case, dr, dtype)
+    loss, parts = replay.oracle_loss(model_key, case, hp, adj, dr, params, st)
+    ue, ie, layers = bpr_tables(model_key, case, hp, adj, dr, params)
+    batch = tuple(torch.from_numpy(case[k]) for k in ('ancs', 'poss', 'negs'))
+    assert torch.equal(bpr_part(model_key, ue, ie, batch), parts['bpr_loss']), 'the tables are not the ones the BPR term read'
+    t = term(ue, ie, layers) / len(case['ancs'])
+    loss = loss - parts.pop('bpr_loss') + t
+    parts[name] = t
+    loss.backward()
+    return dict(loss=float(loss.detach()), parts={k: float(v.detach()) for k, v in parts.items()},
+                grads={k: p.grad.double().numpy() for k, p in params.items()})
+
+
+def train_csr(case):
+    """The training matrix as a sorted int64 CSR (rowptr, cols), the form the candidate draw reads."""
+    order = np.lexsort((case['cols'], case['rows']))
+    rowptr = np.concatenate([[0], np.cumsum(np.bincount(case['rows'], minlength=case['n_user']))]).astype(np.int64)
+    return rowptr, case['cols'][order].astype(np.int64)
+
+
+def mixgcf_pick_check(users, layers, ancs, poss, cands, alpha_t, picks):
+    """The picks of a MixGCF step against float64: ``users`` / ``layers`` the float64 summed user table and item layer rows,
+    ``picks`` [B, L+1] the step's.  Where the best float64 score beats the best other item's by more than PICK_GAP_RTOL of
+    the sum of their |terms| (sum_k |u_k m_k|) the pick must be float64's; -> the fraction of (pair, layer) picks so decided."""
+    a = alpha_t.double()[:, None, :, None]
+    xp = torch.stack([x[poss] for x in layers], 1)[:, None]
+    xc = torch.stack([x[cands] for x in layers], 2)                      # [B, M, L+1, d]
+    m = a * xp + (1 - a) * xc
+    u = users[ancs][:, None, None, :]
+    s, A = (u * m).sum(-1), (u * m).abs().sum(-1)                        # [B, M, L+1]
+    want = mixgcf_oracle.picks(users, layers, ancs, poss, cands, alpha_t)
+    j = s.argmax(1, keepdim=True)
+    other = torch.where(cands[:, :, None] == want[:, None, :], torch.full_like(s, -np.inf), s)    # candidates of other items
+    k = other.argmax(1, keepdim=True)
+    gap = s.gather(1, j) - other.gather(1, k)
+    decided = (gap > PICK_GAP_RTOL * (A.gather(1, j) + A.gather(1, k)))[:, 0]
+    bad = decided & (picks != want)
+    assert not bool(bad.any()), f'{int(bad.sum())} decided picks differ from float64 (first (pair, layer): {bad.nonzero()[0].tolist()})'
+    return float(decided.double().mean())
 
 
 def golden_loss_grads_close(g, loss, parts, named_params, what=''):

@@ -9,9 +9,13 @@ arguments write nothing.
 
 Models (LightGCN, SimGCL, SGL, NCL, HCCF, LightGCL): the key false is the key absent bit for bit; under train.deterministic two
 runs and a CUDA-graph replay are bit-identical; with injected alpha = 0 and M = 1 the loss and gradients equal the plain step
-within fp32 rounding.  LightGCN, SGL and SimGCL: the whole step equals the float64 oracle (oracle/cf_oracle with the injected
-masks and noise, its BPR term replaced by the MixGCF term of tests/mixgcf_oracle on the model's own alpha and picks) within the
-golden tolerances.  SimGCL and NCL resumed from a mid-run checkpoint end bit-identical to an uninterrupted run."""
+within fp32 rounding.  All six, on both gradient routes: the whole step equals the float64 oracle (oracle/cf_oracle with the
+injected masks, noise, k-means state and SVD factors, its BPR term replaced by the MixGCF term of tests/mixgcf_oracle on the
+model's own alpha and picks over the layer tables of ssl_test_helpers.bpr_tables) within the golden tolerances, for every
+parameter's gradient, on the goldens and on the split-hub graph of ssl_test_helpers.path_case at d = 20, 64, 128 (NCL's context
+layer beyond, inside and at the last mixed layer; HCCF at two hyper widths); its picks are float64's wherever the score gap is
+decided.  tests/test_host_mixgcf.py shows on the host that the float32 oracle meets these bounds and slightly wrong MixGCF terms
+do not.  SimGCL and NCL resumed from a mid-run checkpoint end bit-identical to an uninterrupted run."""
 import numpy as np
 import pytest
 import torch
@@ -289,68 +293,86 @@ def test_two_runs_and_graph_replay_are_bit_identical(key):
             assert torch.equal(first[1][n_], other[1][n_]), (key, what, n_)
 
 
-def _golden_model(model_key, case, hp, inject, train):
-    from sslrec_b200.config import configs
-    cfg_train = dict(train)
+def whole_step_rows(ssm: bool):
+    """(model_key, case name, hyper-parameter overrides, dim, M, sampled-softmax tau or None, deterministic) of the whole-step
+    tests: the goldens' ``small`` rows, then every case of ``ssl_test_helpers.bpr_term_cases`` on the default route and, at
+    d = 64, M = 8 and the default tau, on the train.deterministic route too."""
+    tau = H.BPR_TERM_TAU if ssm else None
+    rows = [pytest.param(m, 'small', {}, 64, 8, tau, False, id=f'{m}-small') for m in ('lightgcn', 'simgcl', 'sgl')]
+    for c in H.bpr_term_cases(ssm):
+        m, hp, d, M, t = c
+        for det in (False, True) if (d, M, t) == (64, 8, tau) else (False,):
+            rows.append(pytest.param(m, 'paths', hp, d, M, t, det, id=H.bpr_term_case_id(c) + ('-det' if det else '')))
+    return rows
+
+
+def whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic, train, term_fn, cands_at):
+    """One cal_loss + backward of the model on a golden case or a ``bpr_term_setup`` case, with the draws, NCL's k-means and
+    LightGCL's SVD factors injected (tests/test_gpu_model_paths._gpu_model) and the train keys ``train``; the candidates are
+    captured from ``engine.<term_fn>`` (argument ``cands_at``).  -> (dict(loss, parts, grads) of float64 numpy, the
+    candidates, the model, (case, hp, adj, draws, state))."""
     import sslrec_b200.config as cfgmod
+    from sslrec_b200 import engine as E
+    from test_gpu_model_paths import _batch, _gpu_model
+    if case_name == 'paths':
+        case, hp, adj, dr, st = H.bpr_term_setup(model_key, hp_over, dim)
+    else:
+        hp, case = replay.load_golden(model_key, case_name)['hp'], inputs.make_case(case_name)
+        adj = O.normalized_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
+        dr = replay.draws(model_key, case, hp, adj)
+        st = H.path_state(model_key, case, hp, adj, dr)
+    margin = H.kink_margin(model_key, case, hp, adj, dr, st)
+    assert margin > H.KINK_MARGIN, f'ill-posed case: a kink input within {margin:.2e} of its |term| sum'
     default = cfgmod.default_config
 
     def with_train(name, **kw):
         cfg = default(name, **kw)
-        cfg['train'].update(cfg_train)
+        cfg['train'].update(train, dns_candidates=M, deterministic=deterministic)
         return cfg
 
-    cfgmod.default_config = with_train
-    try:
-        model, dh = H.make_model(model_key, case, hp, inject=inject)
-    finally:
-        cfgmod.default_config = default
-    assert configs['train']['mixgcf'] is True
-    return model
+    monkeypatch.setattr(cfgmod, 'default_config', with_train)
+    model = _gpu_model(model_key, case, hp, adj, dr, st)
+    assert E.deterministic() == deterministic and model.dns_candidates == M
+    seen = {}
+    fn = getattr(E, term_fn)
 
+    def keep(*args):
+        seen['cands'] = args[cands_at].clone()
+        return fn(*args)
 
-def _oracle_layers(model_key, adj, hp, dr, ue, ie):
-    """The item rows of layers 0 .. L of the view the BPR term reads, and its summed user / item tables (float64)."""
-    e0 = torch.cat([ue, ie], 0)
-    if model_key == 'lightgcn':
-        a_t = O.edge_dropped(adj, dr['edge_keep'], hp['keep_rate'], False, ue.dtype)
-    else:                                       # SimGCL's clean view, SGL's keep_rate 1.0 view
-        a_t = adj.torch_coo(ue.dtype)
-    xs = [e0]
-    for _ in range(hp['layer_num']):
-        xs.append(O.propagate(a_t, xs[-1]))
-    e = sum(xs)
-    nu = adj.n_user
-    return [x[nu:] for x in xs], e[:nu], e[nu:]
-
-
-@pytest.mark.parametrize('model_key,case_name', [('lightgcn', 'small'), ('simgcl', 'small'), ('sgl', 'small')])
-def test_whole_step_against_float64(model_key, case_name):
-    g = replay.load_golden(model_key, case_name)
-    hp = g['hp']
-    case = inputs.make_case(case_name)
-    adj = O.normalized_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
-    dr = replay.draws(model_key, case, hp, adj)
-    model = _golden_model(model_key, case, hp, H.gpu_injection(model_key, case, hp, adj, dr), dict(mixgcf=True, dns_candidates=8))
-    model.load_state_dict({'user_embeds': case['user_e'], 'item_embeds': case['item_e']}, strict=False)
-    batch = [torch.from_numpy(case[k]).cuda() for k in ('ancs', 'poss', 'negs')]
+    monkeypatch.setattr(E, term_fn, keep)
     model.zero_grad()
-    loss, parts = model.cal_loss(batch)
+    loss, parts = model.cal_loss(_batch(model_key, case['ancs'], case['poss'], case['negs']))
     loss.backward()
     torch.cuda.synchronize()
+    monkeypatch.undo()
+    got = dict(loss=loss.item(), parts={k: float(v) for k, v in parts.items()},
+               grads={k: p.grad.double().cpu().numpy() for k, p in model.named_parameters()})
+    assert seen['cands'].shape == (len(case['ancs']), M)
+    return got, seen['cands'].cpu(), model, (case, hp, adj, dr, st)
+
+
+@pytest.mark.parametrize('model_key,case_name,hp_over,dim,M,tau,deterministic', whole_step_rows(ssm=False))
+def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, M, tau, deterministic):
+    """The step equals the float64 oracle with its BPR term replaced by mixgcf_oracle.term on the model's own alpha and picks
+    (ssl_test_helpers.bpr_term_oracle): loss, every term and every parameter's gradient within the path_errors bounds; the
+    picks are float64's wherever the score gap is decided (the layer rows the kernel mixed, independently of the backward)."""
+    got, cands, model, (case, hp, adj, dr, st) = whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic,
+                                                            dict(mixgcf=True), 'mixgcf_bpr_sum', 5)
     picks, alpha = model.mixgcf_picks.cpu(), model.mixgcf_alpha.cpu()
-    params = {'user_embeds': case['user_e'].double().requires_grad_(True), 'item_embeds': case['item_e'].double().requires_grad_(True)}
-    ref_total, ref_parts = replay.oracle_loss(model_key, case, hp, adj, dr, params)
-    item_layers, ue, ie = _oracle_layers(model_key, adj, hp, dr, params['user_embeds'], params['item_embeds'])
-    ancs, poss = batch[0].cpu(), batch[1].cpu()
-    mix = X.term(ue, ie, item_layers, ancs, poss, picks, alpha) / ancs.shape[0]
-    ref = ref_total - ref_parts['bpr_loss'] + mix
-    ref.backward()
-    assert abs(loss.item() - ref.item()) <= 1e-5 * max(1.0, abs(ref.item())), (loss.item(), ref.item())
-    assert abs(float(parts['bpr_loss']) - mix.item()) <= 1e-5 * max(1.0, abs(mix.item()))
-    for name in ('user_embeds', 'item_embeds'):
-        want = params[name].grad
-        H.close(getattr(model, name).grad, want, 2e-4, 5e-6 * want.abs().max().item() + 1e-9, f'{model_key} grad {name}')
+    ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
+    ref = H.bpr_term_oracle(model_key, case, hp, adj, dr, st, torch.float64,
+                            lambda u, i, ls: X.term(u, i, ls, ancs, poss, picks, alpha), 'bpr_loss')
+    errs = H.path_errors(got, ref)
+    worst = max(errs, key=errs.get)
+    print(f'mixgcf {model_key}-{case_name}-{hp_over}-d{dim}-M{M}{"-det" if deterministic else ""}: largest error {errs[worst]:.3f} of '
+          f'its bound ({worst})')
+    with torch.no_grad():
+        ue, _, layers = H.bpr_tables(model_key, case, hp, adj, dr, H.path_params(model_key, case, dr, torch.float64))
+    decided = H.mixgcf_pick_check(ue, layers, ancs, poss, cands, alpha, picks)
+    print(f'  picks decided {decided:.4f}')
+    assert decided > 0.9, decided
+    assert errs[worst] <= 1.0, errs
 
 
 @pytest.mark.parametrize('graph', [False, True])

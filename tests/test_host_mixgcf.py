@@ -1,14 +1,18 @@
 """MixGCF negatives (train.mixgcf) without a GPU: the numpy restatement of ssl_mixgcf_bpr_fwd's mixing weights
 (tests/mixgcf_oracle.alpha) against a scalar restatement of the documented draw, the float64 picks and term of the oracle on
 a hand-made case, the key's validation and refusals (a value that is not a bool, DirectAU, more than 8 layers, a row-sharded
-model, data-parallel gradient sync) and the training checkpoint's record of the key."""
+model, data-parallel gradient sync) and the training checkpoint's record of the key.  On every whole-step case of
+tests/test_gpu_mixgcf.py, on host draws: the float32 oracle meets the GPU test's bounds against float64, and three slightly
+wrong MixGCF terms (layers 1 .. L reversed, each layer's gradient routed one layer deeper, the positive's share detached) do not."""
 import types
 
 import numpy as np
 import pytest
 import torch
 
+import dns_oracle as D
 import mixgcf_oracle as X
+import ssl_test_helpers as H
 from oracle import philox as P
 from test_host_resume import make_run
 
@@ -103,3 +107,65 @@ def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
     # a record of a run without either key is what it was before the key existed
     m, tr, _ = make_run('ncl')
     assert not {'mixgcf', 'dns_candidates'} & set(tr._resume_record(m, 'host'))
+
+
+# ---- whole-step cases of tests/test_gpu_mixgcf.py::test_whole_step_against_float64, on host draws ------------------------------
+
+SEED = 0x5EED0123456789AB
+CASES = H.bpr_term_cases(ssm=False)
+
+
+def _host_draws(case, M, L1):
+    """Candidates (tests/dns_oracle on the training CSR) and mixing weights (mixgcf_oracle.alpha) of a case, drawn on the host."""
+    rowptr, cols = H.train_csr(case)
+    cands = D.neg_candidates(case['ancs'], case['negs'], M, rowptr, cols, case['n_item'], SEED)
+    return torch.from_numpy(cands), torch.from_numpy(X.alpha(len(case['ancs']), L1, SEED))
+
+
+def _positive_detached_term(users, items, layers, ancs, poss, pick_ids, alpha_t):
+    """mixgcf_oracle.term with no gradient through the positive's share alpha_l X_l[p] of the mixed negative."""
+    a = alpha_t.to(users.dtype)
+    nhat = sum(a[:, l, None] * x.detach()[poss] + (1 - a[:, l, None]) * x[pick_ids[:, l]] for l, x in enumerate(layers))
+    u = users[ancs]
+    return torch.nn.functional.softplus((u * nhat).sum(1) - (u * items[poss]).sum(1)).sum()
+
+
+def _reversed(layers):
+    """Layers 1 .. L in reverse order."""
+    return layers[:1] + layers[:0:-1]
+
+
+def _one_layer_deeper(layers):
+    """The values of every layer, the gradient of layer l < L routed into layer l + 1."""
+    return [x.detach() + (y - y.detach()) for x, y in zip(layers, layers[1:])] + layers[-1:]
+
+
+@pytest.mark.parametrize('model_key,hp_over,dim,M,tau', CASES, ids=[H.bpr_term_case_id(c) for c in CASES])
+def test_whole_step_float32_meets_the_bounds_and_wrong_oracles_do_not(model_key, hp_over, dim, M, tau):
+    """The float32 oracle is within the GPU test's bounds of float64 on the same picks and alphas, and its picks agree with
+    float64's wherever the gap is decided; each slightly wrong MixGCF term is outside the bounds."""
+    case, hp, adj, dr, st = H.bpr_term_setup(model_key, hp_over, dim)
+    assert H.kink_margin(model_key, case, hp, adj, dr, st) > H.KINK_MARGIN
+    ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
+    cands, alpha = _host_draws(case, M, hp['layer_num'] + 1)
+    tables = {}
+    for dt in (torch.float64, torch.float32):
+        with torch.no_grad():
+            ue, _, layers = H.bpr_tables(model_key, case, hp, adj, dr, H.path_params(model_key, case, dr, dt))
+        tables[dt] = ue.double(), [x.double() for x in layers]
+    (u64, l64), (u32, l32) = tables[torch.float64], tables[torch.float32]
+    picks = X.picks(u64, l64, ancs, poss, cands, alpha)
+    decided = H.mixgcf_pick_check(u64, l64, ancs, poss, cands, alpha, X.picks(u32, l32, ancs, poss, cands, alpha))
+    assert decided > 0.9, decided
+
+    def run(dtype, term=X.term, layers_of=lambda ls: ls):
+        return H.bpr_term_oracle(model_key, case, hp, adj, dr, st, dtype,
+                                 lambda u, i, ls: term(u, i, layers_of(ls), ancs, poss, picks, alpha), 'bpr_loss')
+
+    ref = run(torch.float64)
+    ok = H.path_errors(run(torch.float32), ref)
+    assert max(ok.values()) <= 1.0, ok
+    for what, kw in (('layers 1 .. L reversed', dict(layers_of=_reversed)), ('gradients one layer deeper', dict(layers_of=_one_layer_deeper)),
+                     ('positive share detached', dict(term=_positive_detached_term))):
+        bad = H.path_errors(run(torch.float32, **kw), ref)
+        assert max(bad.values()) > 1.0, (what, bad)

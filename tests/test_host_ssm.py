@@ -1,7 +1,8 @@
 """The sampled softmax loss (train.ssm_temperature) without a GPU: the key's validation and refusals (a value that is not a
 finite number > 0, the key together with train.mixgcf, DirectAU, a row-sharded model, data-parallel gradient sync), the
 training checkpoint's record of the key, and the oracle's identities (M = 1 is softplus(s_0' - s_+); the fp32 restatement
-against float64)."""
+against float64).  On every whole-step case of tests/test_gpu_ssm.py, on host draws: the float32 oracle meets the GPU test's
+bounds against float64, and one at tau (1 + 1e-3) does not."""
 import types
 
 import numpy as np
@@ -9,6 +10,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import dns_oracle as D
+import ssl_test_helpers as H
 import ssm_oracle as S
 from test_host_resume import make_run
 
@@ -125,3 +128,28 @@ def test_fma32_is_exact():
     # exact halfway cases in float32 that float64 rounding alone would break
     x = np.float32(1 + 2 ** -23)
     assert S.fma32(x, x, np.float32(-1)) == np.float32(2 ** -22 + 2 ** -46)
+
+
+# ---- whole-step cases of tests/test_gpu_ssm.py::test_whole_step_against_float64, on host draws ---------------------------------
+
+CASES = H.bpr_term_cases(ssm=True)
+
+
+@pytest.mark.parametrize('model_key,hp_over,dim,M,tau', CASES, ids=[H.bpr_term_case_id(c) for c in CASES])
+def test_whole_step_float32_meets_the_bounds_and_a_wrong_tau_does_not(model_key, hp_over, dim, M, tau):
+    """The float32 oracle is within the GPU test's bounds of float64 on the same candidates (tests/dns_oracle's draw on the
+    training CSR); the oracle at tau (1 + 1e-3) is outside them."""
+    case, hp, adj, dr, st = H.bpr_term_setup(model_key, hp_over, dim)
+    assert H.kink_margin(model_key, case, hp, adj, dr, st) > H.KINK_MARGIN
+    ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
+    rowptr, cols = H.train_csr(case)
+    cands = torch.from_numpy(D.neg_candidates(case['ancs'], case['negs'], M, rowptr, cols, case['n_item'], 0x5EED0123456789AB))
+
+    def run(dtype, t):
+        return H.bpr_term_oracle(model_key, case, hp, adj, dr, st, dtype, lambda u, i, _: S.term64(u, i, ancs, poss, cands, t), 'ssm_loss')
+
+    ref = run(torch.float64, tau)
+    ok = H.path_errors(run(torch.float32, tau), ref)
+    assert max(ok.values()) <= 1.0, ok
+    bad = H.path_errors(run(torch.float32, tau * (1 + 1e-3)), ref)
+    assert max(bad.values()) > 1.0, ('tau * (1 + 1e-3) passes', bad)
