@@ -551,8 +551,8 @@ SSL_API int ssl_mixgcf_bpr_bwd(const float *u_tbl, int64_t u_stride, const float
  *   ssl_ssm_bwd, g = scale * (*gscale) (gscale may be NULL), with float atomics:
  *     g_items[c_q] += g w_q (u^ / tau - s_q c^_q) / n_q        (each q as it comes)
  *     g_users[ancs[b]] += g sum_q w_q (c^_q / tau - s_q u^) / n_u  (summed in q order, added once)
- *   Duplicate candidates are separate terms adding into one row (no de-duplication, no logQ
- *   correction: the sampler is uniform).  Identity ids into -0.0 stages give the per-position
+ *   Duplicate candidates are separate terms adding into one row (no de-duplication; the logQ
+ *   correction of popularity-drawn candidates is ssl_ssm_fwd_logq, a27).  Identity ids into -0.0 stages give the per-position
  *   contributions train.deterministic scatters in order; the numbering is in csrc/ssm.cuh.
  *   1 <= M <= 256; dim a multiple of 4, <= SSL_MAX_DIM; tau finite and > 0; every table and sink
  *   16-byte aligned with a stride (elements) that is a multiple of 4 and >= dim.  n_pairs = 0 is
@@ -565,6 +565,40 @@ SSL_API int ssl_ssm_bwd(const float *u_tbl, int64_t u_stride, const float *i_tbl
                         const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, float tau, const float *s,
                         const float *w, const float *nrm, const float *gscale, float scale, float *g_users, int64_t gu_stride,
                         float *g_items, int64_t gi_stride, void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * a27  (no counterpart: popularity-proportional negative candidates with the logQ-corrected
+ *   sampled softmax, optional key train.neg_popularity = beta with train.dns_candidates = M >= 2)
+ *   Host tables (engine.pop_tables, float64 then fp32 once): w_i = (deg_i + 1)^beta, deg_i the
+ *   count of item i in the training CSR's columns; V_i >= 1 the largest-remainder rounding of
+ *   n_item 2^32 w_i / sum w (sum V = n_item 2^32 exactly); table [n_item] uint2 {thr, alias}, the
+ *   Walker / Vose alias table of V in exact integers (column capacity 2^32; a column its own item
+ *   fills alone has alias = itself); lp[i] = log(V_i / (n_item 2^32));
+ *   lz_pop[u] = log(1 - sum_{i in P_u} V_i / (n_item 2^32)) (the subtraction in integers);
+ *   lz_uni[u] = log(n_item - deg_u); both 0 for a user who has every item; ln_m = fp32(log M).
+ *   ssl_neg_candidates_pop: cands [n_pairs, M] int64.  cands[b, 0] = negs[b]; cands[b, j >= 1]
+ *   from the Philox4x32-10 blocks keyed (seed; b, j, blk, "DNSP"), blk < 64, two draws
+ *   (x, y) = (r.x, r.y), (r.z, r.w) per block: c = (x * n_item) >> 32; item = c if alias[c] == c
+ *   or y < thr[c], else alias[c]; rejected while in users[b]'s sorted training-CSR row; after 128
+ *   draws the last is kept.  bias (nullable) [n_pairs, M] fp32, in this order:
+ *     bias[b, 0] = ln_m - lz_uni[u]          bias[b, j] = (ln_m + lp[cands[b, j]]) - lz_pop[u]
+ *   = ln(M q_j(c_j)), q_j candidate j's proposal restricted to u's non-positives, so
+ *   sum_{q >= 1} exp(s_q - bias[b, q-1]) estimates sum_{i not in P_u} exp(s_i) without bias
+ *   (ignoring the 128-draw cap).  The seed is *seed_ptr when seed_ptr is non-null, else seed.
+ *   2 <= M <= 256; table 8-byte aligned; lp, lz_pop, lz_uni may be NULL when bias is.
+ *   ssl_ssm_fwd_logq: ssl_ssm_fwd on s^_0 = s_0, s^_q = s_q - bias[b, q-1] (q >= 1, one fp32
+ *   subtraction): m, S, loss_b = (m + logf(S)) - s^_0 and w in ssl_ssm_fwd's order on s^; s is
+ *   stored raw, so ssl_ssm_bwd is its backward unchanged (csrc/ssm.cuh).  Arguments and checks as
+ *   ssl_ssm_fwd, bias [n_pairs, M] non-null.  n_pairs = 0 is a no-op for both; rejected
+ *   arguments write nothing.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_neg_candidates_pop(const int64_t *users, const int64_t *negs, int64_t n_pairs, int32_t M, const int32_t *trn_rowptr,
+                                   const int32_t *trn_cols, int64_t n_item, const uint32_t *table, const float *lp,
+                                   const float *lz_pop, const float *lz_uni, float ln_m, uint64_t seed, const uint64_t *seed_ptr,
+                                   int64_t *cands, float *bias, void *stream);
+SSL_API int ssl_ssm_fwd_logq(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
+                             const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, float tau,
+                             float *loss_b, float *s, float *w, float *nrm, const float *bias, void *stream);
 
 #ifdef __cplusplus
 }

@@ -108,6 +108,17 @@ class BaseModel(nn.Module):
             raise ValueError(f'train.ssm_temperature: {type(self).__name__} trains without negatives')
         if self.ssm_temperature is not None and self.mixgcf:
             raise ValueError('train.ssm_temperature and train.mixgcf both replace the BPR term: set one of them')
+        # optional key train.neg_popularity = beta: the candidates 1 .. M-1 of train.dns_candidates are drawn in proportion to
+        # (deg_i + 1)^beta (``_pop_tables``, built once like ``_train_csr``); the sampled softmax loss then takes the logQ
+        # correction ``_ssm_bias`` of the step's candidates
+        self.neg_popularity = E.neg_popularity()
+        self._pop = None
+        self._ssm_bias = None
+        if self.neg_popularity is not None and not self.bpr_negatives:
+            raise ValueError(f'train.neg_popularity: {type(self).__name__} trains without negatives')
+        if self.neg_popularity is not None and self.dns_candidates < 2:
+            raise ValueError('train.neg_popularity draws the candidates of train.dns_candidates, which must then be >= 2, '
+                             f'got {self.dns_candidates}')
 
     bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / mixgcf / ssm_temperature apply)
 
@@ -121,7 +132,8 @@ class BaseModel(nn.Module):
         train.dns_candidates is 1 and neither train.mixgcf nor train.ssm_temperature is set.  Their seed is the last one the step
         draws, so a DNS step draws every seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed,
         and with M = 1 its candidates are the loader's negatives (no draw).  The sampled softmax loss with M = 1 takes the
-        loader's negatives without drawing a seed."""
+        loader's negatives without drawing a seed.  With train.neg_popularity the candidates come from the popularity draw on
+        the same seed, and with the sampled softmax their logQ correction is kept in ``_ssm_bias`` for ``_bpr_term``."""
         from . import engine as E
         if self.dns_candidates == 1 and not self.mixgcf:
             return None if self.ssm_temperature is None else E._i64(negs, ancs.device).view(-1, 1)
@@ -130,7 +142,26 @@ class BaseModel(nn.Module):
         if self.dns_candidates == 1:
             return E._i64(negs, ancs.device).view(-1, 1)
         rowptr, cols = self._train_csr(ancs.device)
-        return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed)
+        if self.neg_popularity is None:
+            return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed)
+        pop = self._pop_tables(ancs.device)
+        if self.ssm_temperature is None:
+            return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed, pop=pop)
+        cands, self._ssm_bias = E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed, pop=pop,
+                                                 want_bias=True)
+        return cands
+
+    def _pop_tables(self, device):
+        """The alias table and logQ tables of train.neg_popularity (``engine.PopTables``) on ``device``, built once from the
+        training CSR ``_train_csr`` uploads: a pure function of (training matrix, beta), so checkpoints do not store it."""
+        from . import engine as E
+        if self._pop is None or self._pop.table.device != device:
+            import numpy as np
+            import scipy.sparse as sp
+            m = sp.csr_matrix(self._trn_mat)
+            m.sort_indices()
+            self._pop = E.PopTables(m.indptr.astype(np.int64), m.indices.astype(np.int64), self.item_num, self.neg_popularity, device)
+        return self._pop
 
     def _bpr_term(self, users, items, item_layers, ancs, poss, negs, cands, bpr):
         """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term; with DNS the term on
@@ -144,7 +175,9 @@ class BaseModel(nn.Module):
                                                                           self._mix_alpha_in)
             return loss, negs
         if self.ssm_temperature is not None:
-            return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature), negs
+            if self.neg_popularity is None:
+                return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature), negs
+            return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature, bias=self._ssm_bias), negs
         rows = isinstance(users, E.Rows)
         if cands is not None:
             negs = self._dns_select(users if rows else users.detach(), items if rows else items.detach(), ancs, cands)
@@ -194,6 +227,8 @@ class BaseModel(nn.Module):
             raise ValueError('train.mixgcf is single-GPU: a row-sharded model does not mix negatives')
         if comm is not None and self.ssm_temperature is not None:
             raise ValueError('train.ssm_temperature is single-GPU: a row-sharded model does not score sampled candidates')
+        if comm is not None and self.neg_popularity is not None:
+            raise ValueError('train.neg_popularity is single-GPU: a row-sharded model does not draw candidates')
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

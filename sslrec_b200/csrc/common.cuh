@@ -5,6 +5,7 @@
 #include <stdio.h>
 
 #include "../../include/sslrec_b200.h"
+#include "csr_contains.cuh"
 #include "philox.cuh"
 
 namespace ssl {
@@ -57,18 +58,6 @@ __host__ __device__ __forceinline__ bool node_keep_rng(uint64_t seed, uint32_t r
 __host__ __device__ __forceinline__ float4 noise_u4_rng(uint64_t seed, uint32_t stream, uint32_t row, uint32_t quad) {
     uint4 r = philox4x32_10(make_uint4(row, quad, stream, 0x4E4F4953u /*"NOIS"*/), seed_key(seed));
     return make_float4(u01(r.x), u01(r.y), u01(r.z), u01(r.w));
-}
-
-// key in the sorted int32 column list cols[lo, hi) (a training-CSR row)?  Binary search; the negative samplers'
-// rejection test (sample_negs_kernel, hard_negs.cu).
-__device__ __forceinline__ bool csr_contains(const int32_t *__restrict__ cols, int lo, int hi, int key) {
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        const int v = __ldg(cols + mid);
-        if (v == key) return true;
-        if (v < key) lo = mid + 1; else hi = mid;
-    }
-    return false;
 }
 
 // 3xTF32 split: hi = round-to-nearest tf32(x), lo = round-to-nearest tf32(x - hi).  Rounding (not

@@ -19,6 +19,10 @@
 // which is lse_q(s_q) - s_0 with x^ = x / sqrt(1e-8 + |x|^2) and s_q = x^_u . x^_q / tau.  The forward writes loss_b [B],
 // s [B, M+1], w [B, M+1] and nrm [B, M+2] (column 0 n_u, column 1 + q n_q), which the backward reads instead of recomputing.
 //
+// logQ-corrected forward (ssm_fwd_logq_kernel, train.neg_popularity): with bias [B, M] (pop_negs.cuh), s^_0 = s_0 and
+// s^_q = s_q - bias[b, q-1] for q >= 1 (one fp32 subtraction); m, S, loss_b and w are the lines above on s^ instead of s, and
+// s is stored raw.  The backward below is then the correct backward unchanged.
+//
 // Backward, with g = scale * (*gscale) (gscale may be null: 1), per pair and in ascending q = 0 .. M:
 //     gw_q = g * w_q      a_q = gw_q / den_q      e_q = (gw_q * s_q) / (n_q * n_q)
 //     row c_q       += fmaf(a_q, u[k], -(e_q * c_q[k]))                        = g w_q (u^ / tau - s_q c^_q) / n_q
@@ -26,8 +30,8 @@
 // and after the last q
 //     row u         += fmaf(-(beta / (n_u * n_u)), u[k], acc[k])                = g sum_q w_q (c^_q / tau - s_q u^) / n_u
 // The candidate and positive rows are added with float atomics as they come (one add per element and q); the user row is
-// kept in registers across the pair and added once.  Duplicate candidates (the sampler is uniform, so a pair can draw an item
-// twice or draw its positive) are separate terms that add into one row: no de-duplication and no logQ correction.
+// kept in registers across the pair and added once.  Duplicate candidates (a pair can draw an item twice or draw its positive)
+// are separate terms that add into one row: no de-duplication; the logQ correction is the logq forward's alone.
 // Run on gathered rows with identity ids (ancs = poss = 0 .. B-1, cands[b, j] = B + b M + j, the gathered item rows
 // [I[poss]; I[cands]] as the item table) into -0.0 stages, it writes each position's contribution once, in this numbering:
 // the user stage holds positions 0 .. B-1 (rows ancs), the item stage 0 .. B-1 (rows poss) and B + b M + j (rows cands[b, j]);
@@ -83,17 +87,21 @@ __device__ __forceinline__ Lane lane_of(int64_t n_pairs, int G) {
     return Lane{b < n_pairs ? b : n_pairs - 1, b < n_pairs, lane % G};
 }
 
-static __global__ void __launch_bounds__(kWarpsPerBlock * 32)
-    ssm_fwd_kernel(const float *__restrict__ u_tbl, int64_t u_stride, const float *__restrict__ i_tbl, int64_t i_stride,
-                   const int64_t *__restrict__ ancs, const int64_t *__restrict__ poss, const int64_t *__restrict__ cands,
-                   int64_t n_pairs, int M, int dim, float tau, float *__restrict__ loss_b, float *s_out, float *__restrict__ w_out,
-                   float *__restrict__ nrm_out) {
+// the forward of one pair; kLogQ: the softmax runs on s^_q = s_q - bias[b, q-1] (q >= 1, one fp32 subtraction; s^_0 = s_0)
+// while s_out keeps the raw s_q (ssm_fwd_logq_kernel)
+template <bool kLogQ>
+__device__ __forceinline__ void ssm_fwd_body(const float *__restrict__ u_tbl, int64_t u_stride, const float *__restrict__ i_tbl,
+                                             int64_t i_stride, const int64_t *__restrict__ ancs, const int64_t *__restrict__ poss,
+                                             const int64_t *__restrict__ cands, const float *__restrict__ bias, int64_t n_pairs, int M,
+                                             int dim, float tau, float *__restrict__ loss_b, float *s_out, float *__restrict__ w_out,
+                                             float *__restrict__ nrm_out) {
     const int G = group_lanes(dim);
     if (((int64_t)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5)) * (32 / G) >= n_pairs) return;   // warp-uniform
     const Lane ln = lane_of(n_pairs, G);
     const int64_t b = ln.b;
     const bool live = ln.slot * 4 < dim;
     const int64_t *cb = cands + b * M;
+    const float *bb = kLogQ ? bias + b * M : nullptr;
     float *sb = s_out + b * (M + 1), *wb = w_out + b * (M + 1), *nb = nrm_out + b * (M + 2);
     const float4 u = load_row(u_tbl, u_stride, __ldg(ancs + b), ln.slot, live);
     const float nu = sqrtf(1e-8f + tree(chain4(u, u), G));
@@ -105,23 +113,45 @@ static __global__ void __launch_bounds__(kWarpsPerBlock * 32)
         const float dt = tree(chain4(u, c), G);
         const float nq = sqrtf(1e-8f + tree(chain4(c, c), G));
         const float s = dt / ((nu * nq) * tau);
-        m = fmaxf(m, s);
+        m = fmaxf(m, kLogQ && q > 0 ? s - __ldg(bb + q - 1) : s);
         if (q == 0) s_pos = s;
         if (ln.active && q % G == ln.slot) {
             sb[q] = s;
             nb[1 + q] = nq;
         }
     }
+    // s^_q, re-formed from the stored raw score by the same subtraction
+    auto shat = [&](int q) { return kLogQ && q > 0 ? sb[q] - __ldg(bb + q - 1) : sb[q]; };
     float part = 0.f;
     if (ln.active)
-        for (int q = ln.slot; q <= M; q += G) part += expf(sb[q] - m);
+        for (int q = ln.slot; q <= M; q += G) part += expf(shat(q) - m);
     const float S = tree(part, G);
     if (!ln.active) return;
-    for (int q = ln.slot; q <= M; q += G) wb[q] = expf(sb[q] - m) / S - (q == 0 ? 1.f : 0.f);
+    for (int q = ln.slot; q <= M; q += G) wb[q] = expf(shat(q) - m) / S - (q == 0 ? 1.f : 0.f);
     if (ln.slot == 0) {
         nb[0] = nu;
         loss_b[b] = (m + logf(S)) - s_pos;
     }
+}
+
+static __global__ void __launch_bounds__(kWarpsPerBlock * 32)
+    ssm_fwd_kernel(const float *__restrict__ u_tbl, int64_t u_stride, const float *__restrict__ i_tbl, int64_t i_stride,
+                   const int64_t *__restrict__ ancs, const int64_t *__restrict__ poss, const int64_t *__restrict__ cands,
+                   int64_t n_pairs, int M, int dim, float tau, float *__restrict__ loss_b, float *s_out, float *__restrict__ w_out,
+                   float *__restrict__ nrm_out) {
+    ssm_fwd_body<false>(u_tbl, u_stride, i_tbl, i_stride, ancs, poss, cands, nullptr, n_pairs, M, dim, tau, loss_b, s_out, w_out,
+                        nrm_out);
+}
+
+// the logQ-corrected forward (ssl_ssm_fwd_logq): bias [n_pairs, M] from ssl_neg_candidates_pop (pop_negs.cuh); the backward
+// is ssm_bwd_kernel unchanged, since the derivative of every s_q needs only the raw s_q and the weight w_q
+static __global__ void __launch_bounds__(kWarpsPerBlock * 32)
+    ssm_fwd_logq_kernel(const float *__restrict__ u_tbl, int64_t u_stride, const float *__restrict__ i_tbl, int64_t i_stride,
+                        const int64_t *__restrict__ ancs, const int64_t *__restrict__ poss, const int64_t *__restrict__ cands,
+                        const float *__restrict__ bias, int64_t n_pairs, int M, int dim, float tau, float *__restrict__ loss_b,
+                        float *s_out, float *__restrict__ w_out, float *__restrict__ nrm_out) {
+    ssm_fwd_body<true>(u_tbl, u_stride, i_tbl, i_stride, ancs, poss, cands, bias, n_pairs, M, dim, tau, loss_b, s_out, w_out,
+                       nrm_out);
 }
 
 static __global__ void __launch_bounds__(kWarpsPerBlock * 32)

@@ -21,6 +21,7 @@ import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1459,20 +1460,124 @@ def dns_candidates() -> int:
     return m
 
 
-def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torch.Tensor, n_item: int, seed) -> torch.Tensor:
+def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torch.Tensor, n_item: int, seed, pop=None,
+                   want_bias: bool = False):
     """[B, m] int64 negative candidates of the pairs (users[b], ., negs[b]) (``ssl_neg_candidates``): column 0 is ``negs``, the
     others are drawn uniformly over the items, rejecting the user's training positives (int32 CSR, sorted rows).  A
-    :class:`DevSeed` passes its device word, so a captured step draws with the seed written there before each replay."""
+    :class:`DevSeed` passes its device word, so a captured step draws with the seed written there before each replay.
+
+    ``pop``: a :class:`PopTables` of the same training CSR draws columns 1 .. m-1 in proportion to the item weights instead
+    (``ssl_neg_candidates_pop``, train.neg_popularity); ``want_bias`` then also returns the [B, m] fp32 logQ correction
+    ln(M q_j(c_j)) of every candidate (include/sslrec_b200.h, a27) as ``(cands, bias)``."""
     dev = trn_cols.device
     users, negs = _i64(users, dev), _i64(negs, dev)
     if negs.numel() != users.numel():
         raise RuntimeError('sslrec_b200: one negative per user')
+    if want_bias and pop is None:
+        raise RuntimeError('sslrec_b200: the logQ correction needs popularity tables')
     cands = torch.empty(users.numel(), int(m), dtype=torch.int64, device=dev)
     with torch.cuda.device(dev):
-        check(lib.ssl_neg_candidates(users.data_ptr(), negs.data_ptr(), users.numel(), int(m), trn_rowptr.data_ptr(), trn_cols.data_ptr(),
-                                     int(n_item), int(seed), getattr(seed, 'ptr', 0) or None, cands.data_ptr(), _stream(cands)),
-              'ssl_neg_candidates')
-    return cands
+        if pop is None:
+            check(lib.ssl_neg_candidates(users.data_ptr(), negs.data_ptr(), users.numel(), int(m), trn_rowptr.data_ptr(),
+                                         trn_cols.data_ptr(), int(n_item), int(seed), getattr(seed, 'ptr', 0) or None, cands.data_ptr(),
+                                         _stream(cands)), 'ssl_neg_candidates')
+            return cands
+        if pop.n_item != int(n_item) or pop.table.device != dev:
+            raise RuntimeError('sslrec_b200: the popularity tables belong to another item set or device')
+        bias = torch.empty(users.numel(), int(m), dtype=torch.float32, device=dev) if want_bias else None
+        check(lib.ssl_neg_candidates_pop(users.data_ptr(), negs.data_ptr(), users.numel(), int(m), trn_rowptr.data_ptr(),
+                                         trn_cols.data_ptr(), int(n_item), pop.table.data_ptr(), pop.lp.data_ptr(), pop.lz_pop.data_ptr(),
+                                         pop.lz_uni.data_ptr(), float(np.float32(math.log(int(m)))), int(seed),
+                                         getattr(seed, 'ptr', 0) or None, cands.data_ptr(), _ptr(bias), _stream(cands)),
+              'ssl_neg_candidates_pop')
+    return (cands, bias) if want_bias else cands
+
+
+# ---- popularity-proportional candidates (optional key train.neg_popularity) --------------------------------------------------
+
+def neg_popularity() -> Optional[float]:
+    """The optional key ``train.neg_popularity`` (INTEGRATION §2): beta, a finite number in [0, 1] (int or float, not a bool);
+    the candidates 1 .. M-1 of train.dns_candidates are then drawn in proportion to (deg_i + 1)^beta (``pop_tables``), and the
+    sampled softmax loss takes the logQ correction.  Absent or null (the default) is the uniform draw.  Raises ValueError for any
+    other value."""
+    from .config import configs
+    b = configs.get('train', {}).get('neg_popularity')
+    if b is None:
+        return None
+    if isinstance(b, bool) or not isinstance(b, (int, float)) or not 0.0 <= b <= 1.0:
+        raise ValueError(f'train.neg_popularity must be a number in [0, 1] or null, got {b!r}')
+    return float(b)
+
+
+def pop_tables(indptr, indices, n_item: int, beta: float) -> dict:
+    """The host tables of the popularity draw (include/sslrec_b200.h, a27) from a training CSR with sorted, distinct columns per
+    row (numpy, float64 and exact integers; a pure function of its arguments):
+
+    ``V`` [n_item] int64: V_i >= 1, the largest-remainder rounding of x_i = n_item 2^32 w_i / sum w, w_i = (deg_i + 1)^beta,
+    deg_i the count of item i in ``indices`` (x_i = (w_i * n_item 2^32) / fsum(w) in float64; the units short of n_item 2^32
+    after the floors go to the largest remainders x_i - floor(x_i), ties to the lower item; a surplus from float64 rounding
+    comes off the smallest remainders the same way), so sum V = n_item 2^32 exactly.
+    ``table`` [n_item, 2] uint32 {thr, alias}: Walker / Vose on V in integers with column capacity 2^32.  Columns start as
+    ``small`` (V < 2^32) and ``large`` (V >= 2^32) stacks in ascending item order; while both are non-empty the top small item
+    s fills its column's share thr = r_s and its alias is the top large item l, whose rest r_l -= 2^32 - r_s moves it to small
+    when below 2^32.  Every item left over then has r = 2^32 exactly: its column is itself alone (alias = itself, thr = 0).
+    ``lp`` [n_item], ``lz_pop`` / ``lz_uni`` [n_user] float32: log(V_i / T), log((T - sum_{i in P_u} V_i) / T) and
+    log(n_item - deg_u), T = n_item 2^32, in float64 rounded once; 0 for a user who has every item."""
+    indptr = np.asarray(indptr, dtype=np.int64)
+    indices = np.asarray(indices, dtype=np.int64)
+    n = int(n_item)
+    if n < 1 or n >= 1 << 31:
+        raise ValueError(f'pop_tables: n_item {n} outside [1, 2^31)')
+    K = 1 << 32
+    T = n * K
+    deg = np.bincount(indices, minlength=n).astype(np.float64)
+    w = (deg + 1.0) ** float(beta)
+    x = (w * float(T)) / math.fsum(w.tolist())
+    fl = np.floor(x)
+    V = fl.astype(np.int64)
+    short = T - int(V.sum())
+    rem = x - fl
+    if short > 0:          # the largest remainders, ties to the lower item (a stable sort of -rem); more than n: whole rounds
+        V += short // n
+        V[np.argsort(-rem, kind='stable')[:short % n]] += 1
+    elif short < 0:
+        V[np.argsort(rem, kind='stable')[:-short]] -= 1
+    if int(V.sum()) != T or int(V.min()) < 1:
+        raise ValueError('pop_tables: the weights do not round to positive integers summing to n_item 2^32')
+    thr = np.zeros(n, dtype=np.uint32)
+    alias = np.arange(n, dtype=np.uint32)
+    r = V.tolist()
+    small = [i for i in range(n) if r[i] < K][::-1]          # stacks: the top (last element) is the lowest item
+    large = [i for i in range(n) if r[i] >= K][::-1]
+    while small and large:
+        s, l = small.pop(), large.pop()
+        thr[s] = r[s]
+        alias[s] = l
+        r[l] -= K - r[s]
+        (small if r[l] < K else large).append(l)
+    if small:                                                # impossible with sum V = n 2^32; kept as a guard
+        raise ValueError('pop_tables: the alias construction did not close')
+    with np.errstate(divide='ignore'):
+        lp = np.log(V.astype(np.float64) / float(T))
+        # sum of V over each user's row, in integers (np.add.reduceat misreads empty rows)
+        cs = np.concatenate([[0], np.cumsum(V[indices])])
+        left = T - (cs[indptr[1:]] - cs[indptr[:-1]])
+        lz_pop = np.where(left > 0, np.log(np.maximum(left, 1).astype(np.float64) / float(T)), 0.0)
+        free = n - np.diff(indptr)
+        lz_uni = np.where(free > 0, np.log(np.maximum(free, 1).astype(np.float64)), 0.0)
+    return {'V': V, 'table': np.stack([thr, alias], 1), 'lp': lp.astype(np.float32), 'lz_pop': lz_pop.astype(np.float32),
+            'lz_uni': lz_uni.astype(np.float32)}
+
+
+class PopTables:
+    """``pop_tables`` on a device: the alias table (int32 [n_item, 2], the uint32 bits of {thr, alias}) and the fp32 ``lp``,
+    ``lz_pop`` and ``lz_uni`` that ``neg_candidates(pop=...)`` reads."""
+
+    def __init__(self, indptr, indices, n_item: int, beta: float, device):
+        h = pop_tables(indptr, indices, n_item, beta)
+        self.n_item, self.beta = int(n_item), float(beta)
+        self.table = torch.from_numpy(np.ascontiguousarray(h['table']).view(np.int32)).to(device)
+        self.lp, self.lz_pop, self.lz_uni = (torch.from_numpy(h[k]).to(device) for k in ('lp', 'lz_pop', 'lz_uni'))
 
 
 def _score_table(t):
@@ -1689,7 +1794,7 @@ class _SsmFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pack, *inputs):
-        ops, ancs, poss, cands, tau, n_plain = pack
+        ops, ancs, poss, cands, tau, bias, n_plain = pack
         users, items = ops
         u_ptr, u_stride, d = _mix_table(users)
         i_ptr, i_stride, d_i = _mix_table(items)
@@ -1702,8 +1807,13 @@ class _SsmFn(torch.autograd.Function):
         s, w, nrm = torch.empty(B, m + 1, **f), torch.empty(B, m + 1, **f), torch.empty(B, m + 2, **f)
         with torch.cuda.device(dev), _timed('ssm_fwd', dict(B=B, M=m, dim=d)):
             st = _stream(cands)
-            check(lib.ssl_ssm_fwd(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(), B, m, d, tau,
-                                  loss_b.data_ptr(), s.data_ptr(), w.data_ptr(), nrm.data_ptr(), st), 'ssl_ssm_fwd')
+            if bias is None:
+                check(lib.ssl_ssm_fwd(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(), B, m, d, tau,
+                                      loss_b.data_ptr(), s.data_ptr(), w.data_ptr(), nrm.data_ptr(), st), 'ssl_ssm_fwd')
+            else:          # the logQ-corrected softmax; s stays raw, so the backward below is the same
+                check(lib.ssl_ssm_fwd_logq(u_ptr, u_stride, i_ptr, i_stride, ancs.data_ptr(), poss.data_ptr(), cands.data_ptr(), B, m, d,
+                                           tau, loss_b.data_ptr(), s.data_ptr(), w.data_ptr(), nrm.data_ptr(), bias.data_ptr(), st),
+                      'ssl_ssm_fwd_logq')
             check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0, out.data_ptr(), st), 'ssl_sum')
         ctx.pack = (ops, ancs, poss, cands, tau, s, w, nrm, n_plain, len(inputs) - n_plain)
         return out
@@ -1744,18 +1854,26 @@ class _SsmFn(torch.autograd.Function):
         return (None,) + tuple(plain_grads[k] for k in range(n_plain)) + (zero,) * n_tokens
 
 
-def ssm_loss_sum(users, items, ancs, poss, cands: torch.Tensor, temp: float) -> torch.Tensor:
+def ssm_loss_sum(users, items, ancs, poss, cands: torch.Tensor, temp: float, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The sampled softmax loss summed over the batch (``ssl_ssm_fwd``; formula in include/sslrec_b200.h, a26): for every pair
     lse_q(s_q) - s_0 over the positive (q = 0) and the candidates ``cands`` [B, M] (column 0 the loader's negative), with
     s_q = cos(users[ancs[b]], items[c_q]) / temp.  ``users`` / ``items`` are each a :class:`Rows` (gradient into its sink; a
     restricted view must mark every candidate row) or a [n, d] fp32 tensor (gradient through autograd, like ``rows_at``); under
-    ``deterministic()`` every batch row's gradient is added in position order."""
+    ``deterministic()`` every batch row's gradient is added in position order.
+
+    ``bias``: the [B, M] fp32 logQ correction of the candidates (``neg_candidates(pop=..., want_bias=True)``): the softmax then
+    runs on s_q - bias[b, q-1] for the candidates (``ssl_ssm_fwd_logq``); no gradient flows into it."""
     dev = cands.device
     ancs, poss, cands = _i64(ancs, dev), _i64(poss, dev), _i64(cands, dev)
     if cands.dim() != 2 or ancs.numel() != cands.shape[0] or poss.numel() != cands.shape[0]:
         raise RuntimeError('sslrec_b200: one anchor, one positive and one row of candidates per pair')
+    if bias is not None:
+        _require_cuda(bias, 'logQ bias')
+        if bias.dtype != torch.float32 or bias.shape != cands.shape:
+            raise RuntimeError('sslrec_b200: the logQ bias must be fp32 and shaped like the candidates')
+        bias = bias.detach().contiguous()
     ops, plain = _mix_operands([users, items])
-    pack = (ops, ancs, poss, cands, float(temp), len(plain))
+    pack = (ops, ancs, poss, cands, float(temp), bias, len(plain))
     return _SsmFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
 
 

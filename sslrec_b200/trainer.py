@@ -109,6 +109,8 @@ class Trainer(object):
             raise ValueError('train.mixgcf is single-GPU: data-parallel ranks share the seed, so their mixing weights would coincide')
         if grad_sync is not None and E.ssm_temperature() is not None:
             raise ValueError('train.ssm_temperature is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
+        if grad_sync is not None and E.neg_popularity() is not None:
+            raise ValueError('train.neg_popularity is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
         self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
@@ -326,6 +328,8 @@ class Trainer(object):
             record['mixgcf'] = True
         if E.ssm_temperature() is not None:
             record['ssm_temperature'] = E.ssm_temperature()
+        if E.neg_popularity() is not None:
+            record['neg_popularity'] = E.neg_popularity()
         return record
 
     def save_checkpoint(self, model, path):
