@@ -1,12 +1,14 @@
 """TEST INFRASTRUCTURE -- restatements of the popularity-proportional candidates (optional key train.neg_popularity), which have
 no counterpart in the reference: the alias-table draw of ssl_neg_candidates_pop in numpy on the Philox blocks of oracle/philox.py,
 its fp32 logQ bias, the logQ-corrected sampled softmax forward (ssl_ssm_fwd_logq) as a sequential float32 restatement on top of
-tests/ssm_oracle, and the distribution an alias table realises, in integers."""
+tests/ssm_oracle, and the distribution an alias table realises, in integers.  In float64 from the definition alone (no integer
+weights, no alias table): the logQ bias (bias64) with its fp32 error bound, and the logQ-corrected term (term64_logq)."""
 from __future__ import annotations
 
 import math
 
 import numpy as np
+import torch
 
 import ssm_oracle as S
 from oracle.philox import philox4x32_10
@@ -70,6 +72,53 @@ def bias(users, cands: np.ndarray, lp, lz_pop, lz_uni) -> np.ndarray:
     out[:, 0] = ln_m - lz_uni[users]
     out[:, 1:] = (ln_m + lp[cands[:, 1:]]).astype(f) - lz_pop[users][:, None]
     return out
+
+
+def _logq64(users, cands, rows, cols, n_user: int, n_item: int, beta: float, m: int):
+    """float64 [B, m] ln q_j(c_j) of the draw's definition and the magnitude of the terms the fp32 bias is formed from."""
+    users, cands = np.asarray(users, np.int64), np.asarray(cands, np.int64)
+    rows, cols = np.asarray(rows, np.int64), np.asarray(cols, np.int64)
+    assert cands.shape == (len(users), m), (cands.shape, len(users), m)
+    assert len(np.unique(rows * n_item + cols)) == len(rows), 'the training pairs must be distinct'
+    w = (np.bincount(cols, minlength=n_item).astype(np.float64) + 1.0) ** float(beta)          # w_i = (deg_i + 1)^beta
+    W = math.fsum(w.tolist())
+    left = np.full(n_user, W)                                                                   # W - sum_{i in P_u} w_i
+    np.subtract.at(left, rows, w[cols])
+    free = n_item - np.bincount(rows, minlength=n_user)                                         # n_item - deg_u
+    assert (free[users] > 0).all(), 'a user with every item has no negative to draw'
+    lq = np.empty(cands.shape, np.float64)
+    mag = np.empty(cands.shape, np.float64)
+    lq[:, 0] = -np.log(free[users])                                                             # column 0: the loader's uniform draw
+    mag[:, 0] = np.log(free[users])
+    lw, lz = np.log(w / W), np.log(left / W)
+    lq[:, 1:] = lw[cands[:, 1:]] - lz[users][:, None]                                           # columns j >= 1: w_c / (W - sum_P w)
+    mag[:, 1:] = np.abs(lw[cands[:, 1:]]) + np.abs(lz[users])[:, None]
+    return lq, mag + math.log(m)
+
+
+def bias64(users, cands, rows, cols, n_user: int, n_item: int, beta: float, m: int) -> np.ndarray:
+    """float64 [B, m] logQ bias ln(M q_j(c_j)) straight from its definition, on the training pairs (rows, cols) (distinct):
+    w_i = (deg_i + 1)^beta; column 0, the loader's uniform negative, q = 1 / (n_item - deg_u); column j >= 1, the popularity
+    draw restricted to the non-positives of u, q = w_c / (W - sum_{i in P_u} w_i), W = sum_i w_i.  Shares nothing with
+    engine.pop_tables (no integer weights, no alias table)."""
+    lq, _ = _logq64(users, cands, rows, cols, n_user, n_item, beta, m)
+    return math.log(m) + lq
+
+
+def bias_tol(users, cands, rows, cols, n_user: int, n_item: int, beta: float, m: int) -> np.ndarray:
+    """float64 [B, m]: the bound on |fp32 bias - bias64|, 2^-21 (ln M + |ln q_pop(c)| + |ln Z_u|) (column 0: ln M + ln(n_item -
+    deg_u)).  The fp32 bias rounds ln M, lp, lz and two sums, each within 2^-24 of a value no larger than that sum; the table's
+    integer weights V_i differ from n_item 2^32 w_i / W by less than one unit, a relative 2^-28 or less on the path graphs."""
+    _, mag = _logq64(users, cands, rows, cols, n_user, n_item, beta, m)
+    return 2.0 ** -21 * mag
+
+
+def term64_logq(users, items, ancs, poss, cands, tau, bias_) -> torch.Tensor:
+    """ssm_oracle.term64 with the candidate scores shifted by the logQ bias: sum_b lse(s_0, s_q - bias[q-1]) - s_0, in the
+    dtype of the tables (``bias_`` [B, M] is cast to it)."""
+    s = S.scores64(users, items, ancs, poss, cands, tau)
+    sh = torch.cat([s[:, :1], s[:, 1:] - torch.as_tensor(bias_).to(s)], 1)
+    return (torch.logsumexp(sh, 1) - s[:, 0]).sum()
 
 
 def forward32_logq(u: np.ndarray, c: np.ndarray, tau: float, bias_: np.ndarray, expf=S.libm_expf, logf=S.libm_logf):

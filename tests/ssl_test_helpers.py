@@ -369,6 +369,25 @@ def train_csr(case):
     return rowptr, case['cols'][order].astype(np.int64)
 
 
+def pop_draw(case, ancs, negs, M, beta, seed):
+    """The train.neg_popularity candidates and fp32 logQ bias a step must draw for the pairs (ancs, ., negs) with ``seed``:
+    tests/pop_oracle's draw and bias on the host tables of the case's own training pairs (``train_csr``) -> ([B, M] int64,
+    [B, M] float32)."""
+    import pop_oracle
+    from sslrec_b200 import engine as E
+    rowptr, cols = train_csr(case)
+    t = E.pop_tables(rowptr, cols, case['n_item'], beta)
+    cands = pop_oracle.neg_candidates(ancs, negs, M, rowptr, cols, case['n_item'], t['table'], int(seed))
+    return cands, pop_oracle.bias(ancs, cands, t['lp'], t['lz_pop'], t['lz_uni'])
+
+
+def assert_step_seed(model):
+    """-> the candidate seed of the model's last step, asserting it is the last seed the step drew from its stream."""
+    seed = int(model._mix_seed)
+    assert seed == model._seeds.state, 'the candidates were not drawn with the step\'s last seed'
+    return seed
+
+
 def mixgcf_pick_check(users, layers, ancs, poss, cands, alpha_t, picks):
     """The picks of a MixGCF step against float64: ``users`` / ``layers`` the float64 summed user table and item layer rows,
     ``picks`` [B, L+1] the step's.  Where the best float64 score beats the best other item's by more than PICK_GAP_RTOL of

@@ -8,7 +8,8 @@ fp32 FMA-chain budget of the float64 maximum and is the exact argmax wherever th
 and rejected arguments.
 
 Models (LightGCN, SimGCL, SGL, NCL, HCCF, LightGCL) under train.deterministic: M = 1 is the plain step bit for bit; an M = 8
-step equals the plain step on the batch whose negatives are the selected ones (``dns_negs``), from the same seed-stream state;
+step equals the plain step on the batch whose negatives are the selected ones (``dns_negs``), from the same seed-stream state,
+with uniform and with popularity candidates (train.neg_popularity), each the oracle's draw for the step's seed bit for bit;
 two runs are identical and a CUDA-graph replay equals the eager loop; SimGCL and SGL mark every candidate row in the restricted
 views; SimGCL and NCL resumed from a mid-run checkpoint end bit-identical to an uninterrupted run."""
 import numpy as np
@@ -222,17 +223,39 @@ def test_m1_is_the_plain_step_bit_for_bit(key):
         _assert_equal(a, b, (key, k))
 
 
-@pytest.mark.parametrize('key', BPR_MODELS)
-def test_dns_step_is_the_plain_step_on_the_selected_negatives(key):
+@pytest.mark.parametrize('key,neg_popularity', [pytest.param(k, b, id=k if b is None else f'{k}-pop{b}')
+                                                 for b in (None, 0.75) for k in BPR_MODELS])
+def test_dns_step_is_the_plain_step_on_the_selected_negatives(monkeypatch, key, neg_popularity):
+    """Also with train.neg_popularity: every step's candidates are the draw of tests/dns_oracle (uniform) or tests/pop_oracle
+    (popularity, on host tables of the case's training pairs) for the step's own pairs and last seed, bit for bit."""
+    import ssl_test_helpers as H
+    from sslrec_b200 import engine as E
     from sslrec_b200.optim import FusedAdam
-    dns, _ = _run(key, 8)
+    dns, _ = _run(key, 8, neg_popularity=neg_popularity)
     plain, _ = _run(key, 1)
     plain.load_state_dict(dns.state_dict())
     od, op = FusedAdam(dns.parameters(), lr=1e-2), FusedAdam(plain.parameters(), lr=1e-2)
+    case = inputs.make_case('tiny')
+    rowptr, cols = H.train_csr(case)
+    seen = {}
+    neg_candidates = E.neg_candidates
+
+    def keep(*args, **kwargs):
+        seen['cands'] = neg_candidates(*args, **kwargs)
+        return seen['cands']
+
+    monkeypatch.setattr(E, 'neg_candidates', keep)
     changed = 0
     for k, batch in enumerate(_batches(key)):
         plain._seeds.load_state_dict(dns._seeds.state_dict())
         a = _step(dns, od, batch)
+        ancs, negs = batch[0].cpu().numpy(), batch[2].cpu().numpy()
+        seed = H.assert_step_seed(dns)
+        if neg_popularity is None:
+            want = D.neg_candidates(ancs, negs, 8, rowptr, cols, case['n_item'], seed)
+        else:
+            want, _ = H.pop_draw(case, ancs, negs, 8, neg_popularity, seed)
+        assert np.array_equal(seen.pop('cands').cpu().numpy(), want), (key, k)
         sel = dns.dns_negs.clone()
         changed += int((sel != batch[2]).sum())
         b = _step(plain, op, [batch[0], batch[1], sel] + batch[3:])

@@ -13,7 +13,8 @@ within fp32 rounding.  All six, on both gradient routes: the whole step equals t
 injected masks, noise, k-means state and SVD factors, its BPR term replaced by the MixGCF term of tests/mixgcf_oracle on the
 model's own alpha and picks over the layer tables of ssl_test_helpers.bpr_tables) within the golden tolerances, for every
 parameter's gradient, on the goldens and on the split-hub graph of ssl_test_helpers.path_case at d = 20, 64, 128 (NCL's context
-layer beyond, inside and at the last mixed layer; HCCF at two hyper widths); its picks are float64's wherever the score gap is
+layer beyond, inside and at the last mixed layer; HCCF at two hyper widths), and at d = 64 with train.neg_popularity, whose
+candidates are tests/pop_oracle's draw for the step's seed bit for bit; its picks are float64's wherever the score gap is
 decided.  tests/test_host_mixgcf.py shows on the host that the float32 oracle meets these bounds and slightly wrong MixGCF terms
 do not.  SimGCL and NCL resumed from a mid-run checkpoint end bit-identical to an uninterrupted run."""
 import numpy as np
@@ -306,11 +307,12 @@ def whole_step_rows(ssm: bool):
     return rows
 
 
-def whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic, train, term_fn, cands_at):
+def whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic, train, term_fn, cands_at, seen=None):
     """One cal_loss + backward of the model on a golden case or a ``bpr_term_setup`` case, with the draws, NCL's k-means and
     LightGCL's SVD factors injected (tests/test_gpu_model_paths._gpu_model) and the train keys ``train``; the candidates are
     captured from ``engine.<term_fn>`` (argument ``cands_at``).  -> (dict(loss, parts, grads) of float64 numpy, the
-    candidates, the model, (case, hp, adj, draws, state))."""
+    candidates, the model, (case, hp, adj, draws, state)).  ``seen``: a dict that also receives the term's ``bias`` keyword
+    (None when it is not passed), as the step passed it."""
     import sslrec_b200.config as cfgmod
     from sslrec_b200 import engine as E
     from test_gpu_model_paths import _batch, _gpu_model
@@ -333,12 +335,13 @@ def whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic
     monkeypatch.setattr(cfgmod, 'default_config', with_train)
     model = _gpu_model(model_key, case, hp, adj, dr, st)
     assert E.deterministic() == deterministic and model.dns_candidates == M
-    seen = {}
+    seen = {} if seen is None else seen
     fn = getattr(E, term_fn)
 
-    def keep(*args):
+    def keep(*args, **kwargs):
         seen['cands'] = args[cands_at].clone()
-        return fn(*args)
+        seen['bias'] = None if kwargs.get('bias') is None else kwargs['bias'].clone()
+        return fn(*args, **kwargs)
 
     monkeypatch.setattr(E, term_fn, keep)
     model.zero_grad()
@@ -352,20 +355,41 @@ def whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic
     return got, seen['cands'].cpu(), model, (case, hp, adj, dr, st)
 
 
-@pytest.mark.parametrize('model_key,case_name,hp_over,dim,M,tau,deterministic', whole_step_rows(ssm=False))
-def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, M, tau, deterministic):
+POP_BETA = 0.75
+
+
+def _mixgcf_rows():
+    """``whole_step_rows(ssm=False)`` with train.neg_popularity absent, then every BPR model at d = 64, M = 8 on both routes
+    with popularity candidates (beta 0.75)."""
+    rows = [pytest.param(*p.values, None, id=p.id) for p in whole_step_rows(ssm=False)]
+    for m, hp in H.BPR_TERM_MODELS:
+        for det in (False, True):
+            rows.append(pytest.param(m, 'paths', hp, 64, 8, None, det, POP_BETA,
+                                     id=H.bpr_term_case_id((m, hp, 64, 8, None)) + ('-det' if det else '') + f'-pop{POP_BETA}'))
+    return rows
+
+
+@pytest.mark.parametrize('model_key,case_name,hp_over,dim,M,tau,deterministic,beta', _mixgcf_rows())
+def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, M, tau, deterministic, beta):
     """The step equals the float64 oracle with its BPR term replaced by mixgcf_oracle.term on the model's own alpha and picks
     (ssl_test_helpers.bpr_term_oracle): loss, every term and every parameter's gradient within the path_errors bounds; the
-    picks are float64's wherever the score gap is decided (the layer rows the kernel mixed, independently of the backward)."""
+    picks are float64's wherever the score gap is decided (the layer rows the kernel mixed, independently of the backward).
+    With train.neg_popularity (``beta``) the candidates are also the popularity draw of tests/pop_oracle for the step's own
+    seed, pairs and training matrix, bit for bit."""
+    train = dict(mixgcf=True) if beta is None else dict(mixgcf=True, neg_popularity=beta)
     got, cands, model, (case, hp, adj, dr, st) = whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic,
-                                                            dict(mixgcf=True), 'mixgcf_bpr_sum', 5)
+                                                            train, 'mixgcf_bpr_sum', 5)
+    if beta is not None:
+        want, _ = H.pop_draw(case, case['ancs'], case['negs'], M, beta, H.assert_step_seed(model))
+        assert np.array_equal(cands.numpy(), want)
     picks, alpha = model.mixgcf_picks.cpu(), model.mixgcf_alpha.cpu()
     ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
     ref = H.bpr_term_oracle(model_key, case, hp, adj, dr, st, torch.float64,
                             lambda u, i, ls: X.term(u, i, ls, ancs, poss, picks, alpha), 'bpr_loss')
     errs = H.path_errors(got, ref)
     worst = max(errs, key=errs.get)
-    print(f'mixgcf {model_key}-{case_name}-{hp_over}-d{dim}-M{M}{"-det" if deterministic else ""}: largest error {errs[worst]:.3f} of '
+    print(f'mixgcf {model_key}-{case_name}-{hp_over}-d{dim}-M{M}{"-det" if deterministic else ""}'
+          f'{"" if beta is None else f"-pop{beta}"}: largest error {errs[worst]:.3f} of '
           f'its bound ({worst})')
     with torch.no_grad():
         ue, _, layers = H.bpr_tables(model_key, case, hp, adj, dr, H.path_params(model_key, case, dr, torch.float64))

@@ -10,7 +10,13 @@ float64, bias = 0 equals ``ssl_ssm_fwd``; rejected arguments write nothing.
 Models (LightGCN, SimGCL, SGL, NCL, HCCF, LightGCL): key null is the key absent bit for bit; with DNS, MixGCF and the sampled
 softmax, two runs and a CUDA-graph replay are bit-identical under train.deterministic; SimGCL's and SGL's restricted views mark
 every candidate; with beta = 0 every bias entry is ln M - ln(n_item - deg_u) and the loss is the uncorrected loss with the
-negative scores shifted by it; SimGCL and NCL resumed from a mid-run checkpoint end bit-identical to an uninterrupted run."""
+negative scores shifted by it; two steps on different batches each apply the bias of their own candidates; SimGCL and NCL resumed
+from a mid-run checkpoint end bit-identical to an uninterrupted run.  All six, on both gradient routes, at beta 0.75 on every
+row of tests/test_gpu_mixgcf.whole_step_rows(ssm=True) and at beta 1 and 0 for LightGCN and HCCF: the step's candidates and
+bias are tests/pop_oracle's for its own seed, pairs and training matrix bit for bit, the bias is within a few ulp of the float64
+bias from its definition, and the whole step equals the float64 oracle with the logQ-corrected term (pop_oracle.term64_logq)
+within the golden tolerances, for every parameter's gradient, while the uncorrected term is outside them;
+tests/test_host_neg_popularity.py shows on the host that the float32 oracle meets these bounds and wrong corrections do not."""
 import math
 
 import numpy as np
@@ -23,6 +29,7 @@ import pop_oracle as O
 import ssl_test_helpers as H
 import ssm_oracle as S
 from test_gpu_hard_negatives import _assert_equal, _batches, _step
+from test_gpu_mixgcf import whole_step, whole_step_rows
 from test_host_resume import make_run
 
 pytestmark = pytest.mark.gpu
@@ -408,6 +415,93 @@ def test_beta_zero_bias_is_the_uniform_correction(monkeypatch, key):
     ref = float((torch.logsumexp(sh, 1) - s[:, 0]).sum())
     B = ancs.numel()
     assert abs(got.item() - ref) <= 1e-5 * max(1.0, abs(ref)) + 4e-7 * B / tau + 2e-6 * B, (got.item(), ref)
+
+
+# ---- whole steps against float64 ---------------------------------------------------------------------------------------------
+
+POP_BETA = 0.75
+
+
+def _whole_step_rows():
+    """Every row of ``test_gpu_mixgcf.whole_step_rows(ssm=True)`` at beta 0.75; LightGCN and HCCF at hyper_num 128 also at beta
+    1 and 0, d = 64, on both routes."""
+    rows = [pytest.param(*p.values, POP_BETA, id=f'{p.id}-beta{POP_BETA}') for p in whole_step_rows(ssm=True)]
+    for m, hp in (('lightgcn', {}), ('hccf', dict(hyper_num=128, keep_rate=0.5))):
+        for beta in (1.0, 0.0):
+            for det in (False, True):
+                rows.append(pytest.param(m, 'paths', hp, 64, 8, H.BPR_TERM_TAU, det, beta, id=H.bpr_term_case_id(
+                    (m, hp, 64, 8, H.BPR_TERM_TAU)) + ('-det' if det else '') + f'-beta{beta}'))
+    return rows
+
+
+@pytest.mark.parametrize('model_key,case_name,hp_over,dim,M,tau,deterministic,beta', _whole_step_rows())
+def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, M, tau, deterministic, beta):
+    """The sampled softmax step with popularity candidates against float64:
+
+    - the candidates and the fp32 bias the term received are tests/pop_oracle's draw and bias for the step's own pairs, last
+      seed and training matrix, bit for bit (so the users are the anchors, column 0 the loader's negative, and the bias is this
+      step's);
+    - that bias is within pop_oracle.bias_tol of bias64, the float64 bias from its definition;
+    - loss, every term and every parameter's gradient are within the path_errors bounds of the float64 oracle whose BPR term is
+      pop_oracle.term64_logq on those candidates and bias64 (ssl_test_helpers.bpr_term_oracle);
+    - the same step is outside those bounds of the uncorrected float64 term, so the correction matters on the row."""
+    seen = {}
+    got, cands, model, (case, hp, adj, dr, st) = whole_step(monkeypatch, model_key, case_name, hp_over, dim, M, deterministic,
+                                                            dict(ssm_temperature=tau, neg_popularity=beta), 'ssm_loss_sum', 4, seen)
+    assert model.neg_popularity == beta and 'bpr_loss' not in got['parts'] and seen['bias'] is not None
+    want, want_bias = H.pop_draw(case, case['ancs'], case['negs'], M, beta, H.assert_step_seed(model))
+    assert np.array_equal(cands.numpy(), want)
+    bias = seen['bias'].cpu().numpy()
+    assert np.array_equal(bias.view(np.uint32), want_bias.view(np.uint32))
+    args = (case['ancs'], want, case['rows'], case['cols'], case['n_user'], case['n_item'], beta, M)
+    b64 = O.bias64(*args)
+    bias_frac = float((np.abs(bias - b64) / O.bias_tol(*args)).max())
+    ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
+
+    def ref(term):
+        return H.bpr_term_oracle(model_key, case, hp, adj, dr, st, torch.float64, term, 'ssm_loss')
+
+    errs = H.path_errors(got, ref(lambda u, i, _: O.term64_logq(u, i, ancs, poss, cands, tau, b64)))
+    plain = H.path_errors(got, ref(lambda u, i, _: S.term64(u, i, ancs, poss, cands, tau)))
+    worst = max(errs, key=errs.get)
+    print(f'neg_popularity {model_key}-{case_name}-{hp_over}-d{dim}-M{M}-tau{tau}-beta{beta}{"-det" if deterministic else ""}: '
+          f'largest error {errs[worst]:.3f} of its bound ({worst}); bias {bias_frac:.3f} of its bound; uncorrected term '
+          f'{max(plain.values()):.3g}x its bound')
+    assert bias_frac <= 1.0, bias_frac
+    assert errs[worst] <= 1.0, errs
+    assert max(plain.values()) > 1.0, ('the uncorrected term passes', plain)
+
+
+@pytest.mark.parametrize('key', BPR_MODELS)
+def test_every_step_applies_its_own_bias(monkeypatch, key):
+    """Two cal_loss calls on different batches: each passes the sampled softmax the bias of its own candidates and users, and
+    its candidates are the draw of its own seed (a bias kept from an earlier step would match the other batch)."""
+    from sslrec_b200 import engine as E
+    from oracle import inputs
+    m, _, _ = make_run(key, device='cuda', train=dict(deterministic=True, ssm_temperature=0.1, dns_candidates=8,
+                                                      neg_popularity=POP_BETA))
+    case = inputs.make_case('tiny')
+    seen = []
+    ssm_loss_sum = E.ssm_loss_sum
+
+    def keep(users, items, ancs, poss, cands, temp, bias=None):
+        seen.append((ancs.clone(), cands.clone(), None if bias is None else bias.clone()))
+        return ssm_loss_sum(users, items, ancs, poss, cands, temp, bias=bias)
+
+    monkeypatch.setattr(E, 'ssm_loss_sum', keep)
+    biases = []
+    for k, batch in enumerate(_batches(key, n=2)):
+        loss, _ = m.cal_loss(batch)
+        loss.backward()
+        torch.cuda.synchronize()
+        assert len(seen) == k + 1
+        ancs, cands, bias = (t.cpu().numpy() for t in seen[k])
+        assert np.array_equal(ancs, batch[0].cpu().numpy())
+        want, want_bias = H.pop_draw(case, ancs, batch[2].cpu().numpy(), 8, POP_BETA, H.assert_step_seed(m))
+        assert np.array_equal(cands, want), k
+        assert np.array_equal(bias.view(np.uint32), want_bias.view(np.uint32)), k
+        biases.append(bias)
+    assert not np.array_equal(*biases)
 
 
 @pytest.mark.parametrize('graph', [False, True])

@@ -7,7 +7,10 @@ equal them exactly; beta = 0 is uniform with every column self-aliased; Zipf-ske
 same table on every call; the per-user tables, a user who has every item included.  The numpy draw oracle (tests/pop_oracle)
 against a scalar restatement of the documented rule and its cap.  The draw kernel and the logQ forward of csrc/ssm.cuh run on the
 host under AddressSanitizer (tests/emu/pop_negs_emu.cpp) and equal the oracle and the float32 restatement bit for bit; with
-bias = 0 the logQ forward equals ssm_fwd_kernel bit for bit."""
+bias = 0 the logQ forward equals ssm_fwd_kernel bit for bit.  On every whole-step case of tests/test_gpu_neg_popularity.py, on
+host draws: the fp32 bias is within pop_oracle.bias_tol of bias64 (beta 0, 0.75 and 1); the float32 oracle with it meets the GPU
+test's bounds against the float64 oracle with bias64, and five wrong corrections (none, column 0 corrected as a popularity
+draw, lz_pop = 0, the bias of permuted anchors, tables of beta 0.7) do not."""
 import math
 import os
 import shutil
@@ -18,7 +21,10 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+import torch
+
 import pop_oracle as O
+import ssl_test_helpers as H
 import ssm_oracle as S
 from oracle import philox as P
 from sslrec_b200 import engine as E
@@ -322,3 +328,71 @@ def test_logq_forward_is_its_restatement_on_the_host(emulator, tmp_path, B, M, d
         assert np.array_equal(g.view(np.uint32), w.view(np.uint32))
     plain = S.forward32(u, c, tau)
     assert np.array_equal(out['bias'][0][1].view(np.uint32), plain[1].ravel().view(np.uint32))
+
+
+# ---- whole-step cases of tests/test_gpu_neg_popularity.py::test_whole_step_against_float64, on host draws ------------------------
+
+CASES = H.bpr_term_cases(ssm=True)
+BETA, SEED = 0.75, 0x5EED0123456789AB
+
+
+def _host_draw(case, M, beta):
+    """The popularity candidates of the case's batch on host tables -> (rowptr, cols, tables, candidates)."""
+    rowptr, cols = H.train_csr(case)
+    t = E.pop_tables(rowptr, cols, case['n_item'], beta)
+    return rowptr, cols, t, O.neg_candidates(case['ancs'], case['negs'], M, rowptr, cols, case['n_item'], t['table'], SEED)
+
+
+@pytest.mark.parametrize('beta', [0.0, BETA, 1.0])
+@pytest.mark.parametrize('model_key,hp_over,dim,M,tau', CASES, ids=[H.bpr_term_case_id(c) for c in CASES])
+def test_fp32_bias_is_within_its_bound_of_bias64(model_key, hp_over, dim, M, tau, beta):
+    case = H.path_case(dim, seed=H.BPR_TERM_SEEDS.get((model_key, dim, hp_over.get('hyper_num')), 41))
+    _, _, t, cands = _host_draw(case, M, beta)
+    b32 = O.bias(case['ancs'], cands, t['lp'], t['lz_pop'], t['lz_uni'])
+    args = (case['ancs'], cands, case['rows'], case['cols'], case['n_user'], case['n_item'], beta, M)
+    frac = np.abs(b32 - O.bias64(*args)) / O.bias_tol(*args)
+    print(f'{H.bpr_term_case_id((model_key, hp_over, dim, M, tau))} beta {beta}: fp32 bias {frac.max():.3f} of its bound')
+    assert frac.max() <= 1.0, frac.max()
+
+
+def _mutations(case, M, t, cands):
+    """Slightly wrong fp32 biases of the same candidates: name -> [B, M] float32, or None for no correction."""
+    ancs = case['ancs']
+    f = np.float32
+    col0_pop = O.bias(ancs, cands, t['lp'], t['lz_pop'], t['lz_uni'])
+    col0_pop[:, 0] = (f(math.log(M)) + t['lp'][case['negs']]).astype(f) - t['lz_pop'][ancs]
+    rowptr, cols = H.train_csr(case)
+    t07 = E.pop_tables(rowptr, cols, case['n_item'], 0.7)
+    return {
+        'no correction': None,
+        'column 0 as a popularity draw': col0_pop,
+        'lz_pop = 0': O.bias(ancs, cands, t['lp'], np.zeros_like(t['lz_pop']), t['lz_uni']),
+        'anchors permuted': O.bias(ancs[np.random.RandomState(7).permutation(len(ancs))], cands, t['lp'], t['lz_pop'], t['lz_uni']),
+        'tables of beta 0.7': O.bias(ancs, cands, t07['lp'], t07['lz_pop'], t07['lz_uni']),
+    }
+
+
+@pytest.mark.parametrize('model_key,hp_over,dim,M,tau', CASES, ids=[H.bpr_term_case_id(c) for c in CASES])
+def test_whole_step_float32_meets_the_bounds_and_wrong_corrections_do_not(model_key, hp_over, dim, M, tau):
+    """The float32 oracle with the fp32 bias of pop_oracle.bias is within the GPU test's bounds of the float64 oracle with
+    bias64 (both on the same host-drawn popularity candidates, beta 0.75); with a wrong bias (none, column 0 corrected as a
+    popularity draw, lz_pop = 0, the bias of permuted anchors, tables of beta 0.7) it is outside them."""
+    case, hp, adj, dr, st = H.bpr_term_setup(model_key, hp_over, dim)
+    assert H.kink_margin(model_key, case, hp, adj, dr, st) > H.KINK_MARGIN
+    ancs, poss = torch.from_numpy(case['ancs']), torch.from_numpy(case['poss'])
+    _, _, t, cands = _host_draw(case, M, BETA)
+    b64 = O.bias64(case['ancs'], cands, case['rows'], case['cols'], case['n_user'], case['n_item'], BETA, M)
+    c = torch.from_numpy(cands)
+
+    def run(dtype, bias):
+        term = ((lambda u, i, _: S.term64(u, i, ancs, poss, c, tau)) if bias is None else
+                (lambda u, i, _: O.term64_logq(u, i, ancs, poss, c, tau, bias)))
+        return H.bpr_term_oracle(model_key, case, hp, adj, dr, st, dtype, term, 'ssm_loss')
+
+    ref = run(torch.float64, b64)
+    ok = max(H.path_errors(run(torch.float32, O.bias(case['ancs'], cands, t['lp'], t['lz_pop'], t['lz_uni'])), ref).values())
+    bad = {name: max(H.path_errors(run(torch.float32, b), ref).values()) for name, b in _mutations(case, M, t, cands).items()}
+    print(f'{H.bpr_term_case_id((model_key, hp_over, dim, M, tau))}: float32 oracle {ok:.3f} of the bound; wrong biases ' +
+          ', '.join(f'{k} {v:.3g}x' for k, v in bad.items()))
+    assert ok <= 1.0, ok
+    assert min(bad.values()) > 1.0, ('a wrong bias passes', bad)
