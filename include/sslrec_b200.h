@@ -42,6 +42,7 @@ extern "C" {
 #define SSL_E_ALLOC (-3)
 
 #define SSL_MAX_VIEWS 4
+#define SSL_MAX_CANDIDATES 256   /* negative candidates per BPR pair (train.dns_candidates) */
 #define SSL_MAX_SUM_SRC 6
 #define SSL_MAX_DIM 128    /* embedding_size must be a multiple of 4 and <= 128 */
 #define SSL_MAX_PEERS 7    /* other GPUs of the node whose tables a kernel stores to over NVLink (8-GPU NVSwitch domain) */

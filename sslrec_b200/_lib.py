@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libsslrec_b200.so')
 
 MAX_VIEWS = 4
+MAX_CANDIDATES = 256
 MAX_SUM_SRC = 6
 MAX_DIM = 128
 MAX_PEERS = 7

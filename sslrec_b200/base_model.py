@@ -3,6 +3,7 @@
 from __future__ import annotations
 
 import ctypes as C
+from typing import NamedTuple, Optional
 
 import torch
 from torch import nn
@@ -10,6 +11,14 @@ from torch import nn
 from ._lib import check, lib
 from .config import configs
 from .graph import GraphPlan
+
+
+class NegDraw(NamedTuple):
+    """A step's candidates (``BaseModel._dns_candidates``): [B, M] int64, column 0 the loader's negatives; the seed they and
+    MixGCF's weights were drawn with (None: no draw); the [B, M] logQ correction of the sampled softmax (None: uncorrected)."""
+    cands: torch.Tensor
+    seed: object
+    bias: Optional[torch.Tensor]
 
 
 class BaseModel(nn.Module):
@@ -84,72 +93,51 @@ class BaseModel(nn.Module):
         # optional: data_handler.plan_source(device, row_ranges, side_split) -> GraphPlan builds the CSR plan without a
         # torch sparse COO tensor (BASELINE config 4: 300 M stored entries are generated and sorted on the device)
         self._plan_source = getattr(data_handler, 'plan_source', None)
-        # optional key train.dns_candidates = M (dynamic negative sampling): >= 2 trains each pair on the highest-scored of M
-        # candidates; ``dns_negs`` then holds the selected negatives of the last step (like ``final_embeds``: last step only)
-        self.dns_candidates = E.dns_candidates()
-        self.dns_negs = None
-        if self.dns_candidates > 1 and not self.bpr_negatives:
-            raise ValueError(f'train.dns_candidates: {type(self).__name__} trains without negatives')
-        # optional key train.mixgcf (MixGCF, with the M candidates of train.dns_candidates): the BPR term's negative is mixed
-        # from the positive and the candidates layer by layer; ``mixgcf_picks`` / ``mixgcf_alpha`` ([B, L+1]) keep the last
-        # step's picked items and mixing weights
-        self.mixgcf = E.mixgcf()
-        self.mixgcf_picks = self.mixgcf_alpha = None
-        self._mix_seed = None
+        # the negative-sampling keys (engine.NegSpec); the last step's outputs: ``dns_negs`` the selected negatives of
+        # train.dns_candidates (like ``final_embeds``: last step only), ``mixgcf_picks`` / ``mixgcf_alpha`` ([B, L+1]) MixGCF's
+        # picked items and mixing weights, ``_mix_seed`` the seed of the candidates and of MixGCF's weights
+        self.neg = E.NegSpec.from_config()
+        self.neg.check_model(self)
+        self.dns_negs = self.mixgcf_picks = self.mixgcf_alpha = self._mix_seed = None
         self._mix_alpha_in = None      # tests: injected [B, L+1] mixing weights instead of the seeded draw
-        if self.mixgcf and not self.bpr_negatives:
-            raise ValueError(f'train.mixgcf: {type(self).__name__} trains without negatives')
-        if self.mixgcf and getattr(self, 'layer_num', 0) + 1 > E.MIXGCF_MAX_LAYERS:
-            raise ValueError(f'train.mixgcf mixes at most {E.MIXGCF_MAX_LAYERS} layers (layer_num + 1), got {self.layer_num + 1}')
-        # optional key train.ssm_temperature = tau (sampled softmax loss, with the M candidates of train.dns_candidates): the BPR
-        # term is replaced by a softmax of the positive against the candidates on cosine scores over tau, reported as ssm_loss
-        self.ssm_temperature = E.ssm_temperature()
-        if self.ssm_temperature is not None and not self.bpr_negatives:
-            raise ValueError(f'train.ssm_temperature: {type(self).__name__} trains without negatives')
-        if self.ssm_temperature is not None and self.mixgcf:
-            raise ValueError('train.ssm_temperature and train.mixgcf both replace the BPR term: set one of them')
-        # optional key train.neg_popularity = beta: the candidates 1 .. M-1 of train.dns_candidates are drawn in proportion to
-        # (deg_i + 1)^beta (``_pop_tables``, built once like ``_train_csr``); the sampled softmax loss then takes the logQ
-        # correction ``_ssm_bias`` of the step's candidates
-        self.neg_popularity = E.neg_popularity()
-        self._pop = None
-        self._ssm_bias = None
-        if self.neg_popularity is not None and not self.bpr_negatives:
-            raise ValueError(f'train.neg_popularity: {type(self).__name__} trains without negatives')
-        if self.neg_popularity is not None and self.dns_candidates < 2:
-            raise ValueError('train.neg_popularity draws the candidates of train.dns_candidates, which must then be >= 2, '
-                             f'got {self.dns_candidates}')
+        self._pop = None               # engine.PopTables of train.neg_popularity, built once (``_pop_tables``)
 
     bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / mixgcf / ssm_temperature apply)
+    # the keys of ``neg`` under their config names, read-only
+    dns_candidates = property(lambda self: self.neg.candidates)
+    mixgcf = property(lambda self: self.neg.mixgcf)
+    ssm_temperature = property(lambda self: self.neg.ssm_temperature)
+    neg_popularity = property(lambda self: self.neg.popularity)
 
     @property
     def bpr_loss_name(self) -> str:
         """The name ``cal_loss`` reports the BPR term under: 'ssm_loss' when train.ssm_temperature replaces it, else 'bpr_loss'."""
-        return 'bpr_loss' if self.ssm_temperature is None else 'ssm_loss'
+        return 'bpr_loss' if self.neg.ssm_temperature is None else 'ssm_loss'
 
-    def _dns_candidates(self, ancs, negs):
-        """The batch's [B, M] DNS candidates (``engine.neg_candidates``; column 0 = the loader's ``negs``), or None when
-        train.dns_candidates is 1 and neither train.mixgcf nor train.ssm_temperature is set.  Their seed is the last one the step
-        draws, so a DNS step draws every seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed,
-        and with M = 1 its candidates are the loader's negatives (no draw).  The sampled softmax loss with M = 1 takes the
-        loader's negatives without drawing a seed.  With train.neg_popularity the candidates come from the popularity draw on
-        the same seed, and with the sampled softmax their logQ correction is kept in ``_ssm_bias`` for ``_bpr_term``."""
+    def _dns_candidates(self, ancs, negs) -> Optional[NegDraw]:
+        """The batch's negative candidates as a ``NegDraw``, or None for the plain step (train.dns_candidates 1, neither
+        train.mixgcf nor train.ssm_temperature).  Their seed, kept as ``_mix_seed``, is the last one the step draws, so a DNS
+        step draws every seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed, and with
+        M = 1 its candidates are the loader's negatives (no draw).  The sampled softmax loss with M = 1 takes the loader's
+        negatives without drawing a seed.  With train.neg_popularity the candidates come from the popularity draw on the same seed, and
+        with the sampled softmax the draw also returns their logQ correction."""
         from . import engine as E
-        if self.dns_candidates == 1 and not self.mixgcf:
-            return None if self.ssm_temperature is None else E._i64(negs, ancs.device).view(-1, 1)
-        seed = self._seeds.next()
-        self._mix_seed = seed
-        if self.dns_candidates == 1:
-            return E._i64(negs, ancs.device).view(-1, 1)
-        rowptr, cols = self._train_csr(ancs.device)
-        if self.neg_popularity is None:
-            return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed)
-        pop = self._pop_tables(ancs.device)
-        if self.ssm_temperature is None:
-            return E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed, pop=pop)
-        cands, self._ssm_bias = E.neg_candidates(ancs, negs, self.dns_candidates, rowptr, cols, self.item_num, seed, pop=pop,
-                                                 want_bias=True)
-        return cands
+        neg = self.neg
+        if neg.candidates == 1 and not neg.mixgcf:
+            if neg.ssm_temperature is None:
+                return None
+            seed = None
+        else:
+            seed = self._mix_seed = self._seeds.next()
+        if neg.candidates == 1:
+            cands, bias = E._i64(negs, ancs.device).view(-1, 1), None
+        else:
+            rowptr, cols = self._train_csr(ancs.device)
+            pop = None if neg.popularity is None else self._pop_tables(ancs.device)
+            want_bias = pop is not None and neg.ssm_temperature is not None
+            out = E.neg_candidates(ancs, negs, neg.candidates, rowptr, cols, self.item_num, seed, pop=pop, want_bias=want_bias)
+            cands, bias = out if want_bias else (out, None)
+        return NegDraw(cands, seed, bias)
 
     def _pop_tables(self, device):
         """The alias table and logQ tables of train.neg_popularity (``engine.PopTables``) on ``device``, built once from the
@@ -160,27 +148,27 @@ class BaseModel(nn.Module):
             import scipy.sparse as sp
             m = sp.csr_matrix(self._trn_mat)
             m.sort_indices()
-            self._pop = E.PopTables(m.indptr.astype(np.int64), m.indices.astype(np.int64), self.item_num, self.neg_popularity, device)
+            self._pop = E.PopTables(m.indptr.astype(np.int64), m.indices.astype(np.int64), self.item_num, self.neg.popularity, device)
         return self._pop
 
-    def _bpr_term(self, users, items, item_layers, ancs, poss, negs, cands, bpr):
-        """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term; with DNS the term on
-        the selected candidates (which the other terms then read too); with MixGCF ``engine.mixgcf_bpr_sum`` and with
-        train.ssm_temperature ``engine.ssm_loss_sum`` on the candidates (the other terms keep the loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors;
-        ``item_layers()`` lists the item rows of its layers 0 .. L (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the
-        plain and DNS terms call (a model passes its module's, so a restatement can stand in for it)."""
+    def _bpr_term(self, users, items, item_layers, ancs, poss, negs, draw, bpr):
+        """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term (``draw`` None); with DNS
+        the term on the selected candidates of ``draw`` (which the other terms then read too); with MixGCF
+        ``engine.mixgcf_bpr_sum`` and with train.ssm_temperature ``engine.ssm_loss_sum`` on them (the other terms keep the
+        loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors; ``item_layers()`` lists the
+        item rows of its layers 0 .. L (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the plain and DNS terms call
+        (a model passes its module's, so a restatement can stand in for it)."""
         from . import engine as E
-        if self.mixgcf:
-            loss, self.mixgcf_picks, self.mixgcf_alpha = E.mixgcf_bpr_sum(users, items, item_layers(), ancs, poss, cands, self._mix_seed,
-                                                                          self._mix_alpha_in)
-            return loss, negs
-        if self.ssm_temperature is not None:
-            if self.neg_popularity is None:
-                return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature), negs
-            return E.ssm_loss_sum(users, items, ancs, poss, cands, self.ssm_temperature, bias=self._ssm_bias), negs
         rows = isinstance(users, E.Rows)
-        if cands is not None:
-            negs = self._dns_select(users if rows else users.detach(), items if rows else items.detach(), ancs, cands)
+        if draw is not None:
+            if self.neg.mixgcf:
+                loss, self.mixgcf_picks, self.mixgcf_alpha = E.mixgcf_bpr_sum(users, items, item_layers(), ancs, poss, draw.cands,
+                                                                              draw.seed, self._mix_alpha_in)
+                return loss, negs
+            if self.neg.ssm_temperature is not None:
+                logq = {} if draw.bias is None else dict(bias=draw.bias)      # uniform candidates: the uncorrected term
+                return E.ssm_loss_sum(users, items, ancs, poss, draw.cands, self.neg.ssm_temperature, **logq), negs
+            negs = self._dns_select(users if rows else users.detach(), items if rows else items.detach(), ancs, draw.cands)
         if rows:
             return bpr(users, items, ancs, poss, negs), negs
         at = E.rows_at          # table[ids]; under train.deterministic with an ordered backward
@@ -221,14 +209,8 @@ class BaseModel(nn.Module):
         from . import engine as E
         if comm is not None and E.deterministic():
             raise RuntimeError('train.deterministic is single-GPU: a row-sharded model sums its partials across GPUs in an order of its own')
-        if comm is not None and self.dns_candidates > 1:
-            raise ValueError('train.dns_candidates is single-GPU: a row-sharded model does not select hard negatives')
-        if comm is not None and self.mixgcf:
-            raise ValueError('train.mixgcf is single-GPU: a row-sharded model does not mix negatives')
-        if comm is not None and self.ssm_temperature is not None:
-            raise ValueError('train.ssm_temperature is single-GPU: a row-sharded model does not score sampled candidates')
-        if comm is not None and self.neg_popularity is not None:
-            raise ValueError('train.neg_popularity is single-GPU: a row-sharded model does not draw candidates')
+        if comm is not None:
+            self.neg.refuse_multi_gpu(sharded=True)
         self.comm = comm
         self._plans.clear()
         if comm is None or not comm.shard_propagation:

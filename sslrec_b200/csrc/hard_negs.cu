@@ -51,7 +51,7 @@ extern "C" int ssl_neg_candidates(const int64_t *users, const int64_t *negs, int
                                   const int32_t *trn_cols, int64_t n_item, uint64_t seed, const uint64_t *seed_ptr, int64_t *cands,
                                   void *stream) {
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31) && n_item > 0 && n_item < (1ll << 31), "ssl_neg_candidates: bad sizes");
-    SSL_CHECK_ARG(M >= 2 && M <= ssl_dns::kMaxCandidates, "ssl_neg_candidates: M = %d outside [2, %d]", M, ssl_dns::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 2 && M <= SSL_MAX_CANDIDATES, "ssl_neg_candidates: M = %d outside [2, %d]", M, SSL_MAX_CANDIDATES);
     if (n_pairs == 0) return SSL_OK;
     SSL_CHECK_ARG(users && negs && trn_rowptr && trn_cols && cands, "ssl_neg_candidates: null pointer");
     const int64_t total = n_pairs * M;
@@ -64,7 +64,7 @@ extern "C" int ssl_neg_candidates(const int64_t *users, const int64_t *negs, int
 extern "C" int ssl_neg_select(const float *u_tbl, int64_t u_stride, const float *i_tbl, int64_t i_stride, const int64_t *ancs,
                               const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, int64_t *negs_out, void *stream) {
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31), "ssl_neg_select: %lld pairs", (long long)n_pairs);
-    SSL_CHECK_ARG(M >= 2 && M <= ssl_dns::kMaxCandidates, "ssl_neg_select: M = %d outside [2, %d]", M, ssl_dns::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 2 && M <= SSL_MAX_CANDIDATES, "ssl_neg_select: M = %d outside [2, %d]", M, SSL_MAX_CANDIDATES);
     SSL_CHECK_ARG(dim >= 1 && dim <= SSL_MAX_DIM, "ssl_neg_select: dim %d out of range", dim);
     SSL_CHECK_ARG(u_stride >= dim && i_stride >= dim, "ssl_neg_select: a stride is below dim %d", dim);
     if (n_pairs == 0) return SSL_OK;

@@ -20,7 +20,6 @@
 namespace ssl_dns {
 
 constexpr int kWarpsPerBlock = 8;
-constexpr int kMaxCandidates = 256;
 
 static __global__ void __launch_bounds__(kWarpsPerBlock * 32)
     neg_select_kernel(const float *__restrict__ u_tbl, int64_t u_stride, const float *__restrict__ i_tbl, int64_t i_stride,

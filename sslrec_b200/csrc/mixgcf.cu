@@ -11,7 +11,7 @@ extern "C" int ssl_mixgcf_bpr_fwd(const float *u_tbl, int64_t u_stride, const fl
                                   float *alpha_out, float *nhat, void *stream) {
     namespace X = ssl_mix;
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31), "ssl_mixgcf_bpr_fwd: %lld pairs", (long long)n_pairs);
-    SSL_CHECK_ARG(M >= 1 && M <= X::kMaxCandidates, "ssl_mixgcf_bpr_fwd: M = %d outside [1, %d]", M, X::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 1 && M <= SSL_MAX_CANDIDATES, "ssl_mixgcf_bpr_fwd: M = %d outside [1, %d]", M, SSL_MAX_CANDIDATES);
     SSL_CHECK_ARG(n_layers >= 1 && n_layers <= X::kMaxLayers, "ssl_mixgcf_bpr_fwd: %d layers outside [1, %d]", n_layers, X::kMaxLayers);
     SSL_CHECK_ARG(dim >= 1 && dim <= SSL_MAX_DIM, "ssl_mixgcf_bpr_fwd: dim %d out of range", dim);
     SSL_CHECK_ARG(u_stride >= dim && i_stride >= dim, "ssl_mixgcf_bpr_fwd: a stride is below dim %d", dim);

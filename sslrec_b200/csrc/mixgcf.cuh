@@ -43,7 +43,6 @@ namespace ssl_mix {
 
 constexpr int kWarpsPerBlock = 8;
 constexpr int kMaxLayers = 8;
-constexpr int kMaxCandidates = 256;
 constexpr uint32_t kTagAlpha = 0x4D495841u;   // "MIXA"
 
 // the item rows of layers 0 .. n_layers-1; a __grid_constant__ kernel parameter, so indexing it by layer reads the parameter

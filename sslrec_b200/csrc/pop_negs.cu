@@ -10,7 +10,7 @@ extern "C" int ssl_neg_candidates_pop(const int64_t *users, const int64_t *negs,
                                       int64_t *cands, float *bias, void *stream) {
     namespace P = ssl_pop;
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31) && n_item > 0 && n_item < (1ll << 31), "ssl_neg_candidates_pop: bad sizes");
-    SSL_CHECK_ARG(M >= 2 && M <= P::kMaxCandidates, "ssl_neg_candidates_pop: M = %d outside [2, %d]", M, P::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 2 && M <= SSL_MAX_CANDIDATES, "ssl_neg_candidates_pop: M = %d outside [2, %d]", M, SSL_MAX_CANDIDATES);
     if (n_pairs == 0) return SSL_OK;
     SSL_CHECK_ARG(users && negs && trn_rowptr && trn_cols && table && cands, "ssl_neg_candidates_pop: null pointer");
     SSL_CHECK_ARG(bias == nullptr || (lp && lz_pop && lz_uni), "ssl_neg_candidates_pop: a bias needs lp, lz_pop and lz_uni");

@@ -31,7 +31,6 @@
 namespace ssl_pop {
 
 constexpr int kThreadsPerBlock = 256;
-constexpr int kMaxCandidates = 256;
 constexpr uint32_t kTagCandidates = 0x444E5350u;   // "DNSP"
 
 // the item of one draw (x, y) from column c = (x * n_item) >> 32

@@ -13,7 +13,7 @@ extern "C" int ssl_ssm_fwd(const float *u_tbl, int64_t u_stride, const float *i_
                            float *s, float *w, float *nrm, void *stream) {
     namespace X = ssl_ssm;
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31), "ssl_ssm_fwd: %lld pairs", (long long)n_pairs);
-    SSL_CHECK_ARG(M >= 1 && M <= X::kMaxCandidates, "ssl_ssm_fwd: M = %d outside [1, %d]", M, X::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 1 && M <= SSL_MAX_CANDIDATES, "ssl_ssm_fwd: M = %d outside [1, %d]", M, SSL_MAX_CANDIDATES);
     SSL_CHECK_ARG(dim >= 4 && dim <= SSL_MAX_DIM && dim % 4 == 0, "ssl_ssm_fwd: dim %d is not a multiple of 4 in [4, %d]", dim, SSL_MAX_DIM);
     SSL_CHECK_ARG(u_stride >= dim && i_stride >= dim && u_stride % 4 == 0 && i_stride % 4 == 0,
                   "ssl_ssm_fwd: a stride is below dim %d or not a multiple of 4", dim);
@@ -33,7 +33,7 @@ extern "C" int ssl_ssm_fwd_logq(const float *u_tbl, int64_t u_stride, const floa
                                 float *loss_b, float *s, float *w, float *nrm, const float *bias, void *stream) {
     namespace X = ssl_ssm;
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31), "ssl_ssm_fwd_logq: %lld pairs", (long long)n_pairs);
-    SSL_CHECK_ARG(M >= 1 && M <= X::kMaxCandidates, "ssl_ssm_fwd_logq: M = %d outside [1, %d]", M, X::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 1 && M <= SSL_MAX_CANDIDATES, "ssl_ssm_fwd_logq: M = %d outside [1, %d]", M, SSL_MAX_CANDIDATES);
     SSL_CHECK_ARG(dim >= 4 && dim <= SSL_MAX_DIM && dim % 4 == 0, "ssl_ssm_fwd_logq: dim %d is not a multiple of 4 in [4, %d]", dim,
                   SSL_MAX_DIM);
     SSL_CHECK_ARG(u_stride >= dim && i_stride >= dim && u_stride % 4 == 0 && i_stride % 4 == 0,
@@ -55,7 +55,7 @@ extern "C" int ssl_ssm_bwd(const float *u_tbl, int64_t u_stride, const float *i_
                            float *g_items, int64_t gi_stride, void *stream) {
     namespace X = ssl_ssm;
     SSL_CHECK_ARG(n_pairs >= 0 && n_pairs < (1ll << 31), "ssl_ssm_bwd: %lld pairs", (long long)n_pairs);
-    SSL_CHECK_ARG(M >= 1 && M <= X::kMaxCandidates, "ssl_ssm_bwd: M = %d outside [1, %d]", M, X::kMaxCandidates);
+    SSL_CHECK_ARG(M >= 1 && M <= SSL_MAX_CANDIDATES, "ssl_ssm_bwd: M = %d outside [1, %d]", M, SSL_MAX_CANDIDATES);
     SSL_CHECK_ARG(dim >= 4 && dim <= SSL_MAX_DIM && dim % 4 == 0, "ssl_ssm_bwd: dim %d is not a multiple of 4 in [4, %d]", dim, SSL_MAX_DIM);
     SSL_CHECK_ARG(u_stride >= dim && i_stride >= dim && gu_stride >= dim && gi_stride >= dim && u_stride % 4 == 0 && i_stride % 4 == 0 &&
                       gu_stride % 4 == 0 && gi_stride % 4 == 0,

@@ -51,7 +51,6 @@
 namespace ssl_ssm {
 
 constexpr int kWarpsPerBlock = 8;
-constexpr int kMaxCandidates = 256;
 
 // G: lanes per pair for a row of dim floats
 __host__ __device__ __forceinline__ int group_lanes(int dim) {

@@ -1445,19 +1445,88 @@ def dense_infonce_spec_nodes_mean_dev(embeds1, embeds2, ids, temp):
     return _DenseInfoNceFn.apply(embeds1, embeds2, embeds2, nodes, nodes, float(temp), 1, True, 1e-8, True, False, count)
 
 
-# ---- dynamic negative sampling (optional key train.dns_candidates) ----------------------------------------------------------
+# ---- negative sampling of the BPR models (optional keys train.dns_candidates, mixgcf, ssm_temperature, neg_popularity) -------
 
-DNS_MAX_CANDIDATES = 256
+_SHARED_SEED = 'data-parallel ranks share the seed, so their candidate draws would coincide'
+# why each key is single-GPU: (for a row-sharded model, for data-parallel gradient sync)
+_SINGLE_GPU = {
+    'dns_candidates': ('a row-sharded model does not select hard negatives', _SHARED_SEED),
+    'mixgcf': ('a row-sharded model does not mix negatives', 'data-parallel ranks share the seed, so their mixing weights would coincide'),
+    'ssm_temperature': ('a row-sharded model does not score sampled candidates', _SHARED_SEED),
+    'neg_popularity': ('a row-sharded model does not draw candidates', _SHARED_SEED),
+}
 
 
-def dns_candidates() -> int:
-    """The optional key ``train.dns_candidates`` (INTEGRATION §2): M, the candidates per BPR pair, an integer in [1, 256];
-    1 (the default) is the plain step.  Raises ValueError for any other value."""
-    from .config import configs
-    m = configs.get('train', {}).get('dns_candidates', 1)
-    if isinstance(m, bool) or not isinstance(m, int) or not 1 <= m <= DNS_MAX_CANDIDATES:
-        raise ValueError(f'train.dns_candidates must be an integer in [1, {DNS_MAX_CANDIDATES}], got {m!r}')
-    return m
+@dataclass(frozen=True)
+class NegSpec:
+    """The negative-sampling keys of the train section (INTEGRATION §2); the only reader of them.
+    ``candidates`` (train.dns_candidates): M, the candidates per BPR pair, an integer in [1, 256]; 1 (the default) is the plain
+    step, >= 2 trains each pair on the highest-scored of M (``neg_candidates``, ``hard_negatives``).
+    ``mixgcf`` (train.mixgcf): True replaces the BPR term's negative by MixGCF's mixed negative (``mixgcf_bpr_sum``).
+    ``ssm_temperature`` (train.ssm_temperature): tau, a finite number > 0 (int or float, not a bool), replaces the BPR term by
+    the sampled softmax loss on cosine scores over tau (``ssm_loss_sum``).
+    ``popularity`` (train.neg_popularity): beta, a number in [0, 1] (int or float, not a bool); the candidates 1 .. M-1 are then
+    drawn in proportion to (deg_i + 1)^beta (``pop_tables``), and the sampled softmax takes their logQ correction.
+    The two numbers are None when absent or null (the default)."""
+    candidates: int = 1
+    mixgcf: bool = False
+    ssm_temperature: Optional[float] = None
+    popularity: Optional[float] = None
+
+    @classmethod
+    def from_config(cls) -> 'NegSpec':
+        """The keys of ``configs['train']``, each checked on its own: ValueError outside its domain (tau's is checked in fp32)."""
+        from .config import configs
+        t = configs.get('train', {})
+        m = t.get('dns_candidates', 1)
+        if isinstance(m, bool) or not isinstance(m, int) or not 1 <= m <= _lib.MAX_CANDIDATES:
+            raise ValueError(f'train.dns_candidates must be an integer in [1, {_lib.MAX_CANDIDATES}], got {m!r}')
+        on = t.get('mixgcf', False)
+        if not isinstance(on, bool):
+            raise ValueError(f'train.mixgcf must be true or false, got {on!r}')
+        tau = t.get('ssm_temperature')
+        if tau is not None and (isinstance(tau, bool) or not isinstance(tau, (int, float)) or not 0.0 < C.c_float(tau).value < math.inf):
+            raise ValueError(f'train.ssm_temperature must be a finite number > 0 or null, got {tau!r}')
+        beta = t.get('neg_popularity')
+        if beta is not None and (isinstance(beta, bool) or not isinstance(beta, (int, float)) or not 0.0 <= beta <= 1.0):
+            raise ValueError(f'train.neg_popularity must be a number in [0, 1] or null, got {beta!r}')
+        return cls(m, on, None if tau is None else float(tau), None if beta is None else float(beta))
+
+    def record(self) -> dict:
+        """The keys that are set, under their config names and in the order above: what a training checkpoint records.  A key
+        is set when M > 1, MixGCF is on or a number is given, so a run without any of them keeps the record it had before."""
+        rec = {}
+        if self.candidates > 1:
+            rec['dns_candidates'] = self.candidates
+        if self.mixgcf:
+            rec['mixgcf'] = True
+        if self.ssm_temperature is not None:
+            rec['ssm_temperature'] = self.ssm_temperature
+        if self.popularity is not None:
+            rec['neg_popularity'] = self.popularity
+        return rec
+
+    def refuse_multi_gpu(self, sharded: bool) -> None:
+        """Raise ValueError naming the first set key: every key is single-GPU, for a row-sharded model (``sharded``) and for
+        data-parallel gradient sync alike."""
+        key = next(iter(self.record()), None)
+        if key is not None:
+            raise ValueError(f'train.{key} is single-GPU: {_SINGLE_GPU[key][0 if sharded else 1]}')
+
+    def check_model(self, model) -> None:
+        """The rules that involve the model or two keys, in this order: a model without a BPR term (``bpr_negatives`` False)
+        takes none of the keys; MixGCF mixes at most MIXGCF_MAX_LAYERS layers; the sampled softmax and MixGCF both replace the
+        BPR term; the popularity draw needs M >= 2."""
+        key = next(iter(self.record()), None)
+        if key is not None and not model.bpr_negatives:
+            raise ValueError(f'train.{key}: {type(model).__name__} trains without negatives')
+        if self.mixgcf and getattr(model, 'layer_num', 0) + 1 > MIXGCF_MAX_LAYERS:
+            raise ValueError(f'train.mixgcf mixes at most {MIXGCF_MAX_LAYERS} layers (layer_num + 1), got {model.layer_num + 1}')
+        if self.ssm_temperature is not None and self.mixgcf:
+            raise ValueError('train.ssm_temperature and train.mixgcf both replace the BPR term: set one of them')
+        if self.popularity is not None and self.candidates < 2:
+            raise ValueError('train.neg_popularity draws the candidates of train.dns_candidates, which must then be >= 2, '
+                             f'got {self.candidates}')
 
 
 def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torch.Tensor, n_item: int, seed, pop=None,
@@ -1494,20 +1563,6 @@ def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torc
 
 
 # ---- popularity-proportional candidates (optional key train.neg_popularity) --------------------------------------------------
-
-def neg_popularity() -> Optional[float]:
-    """The optional key ``train.neg_popularity`` (INTEGRATION §2): beta, a finite number in [0, 1] (int or float, not a bool);
-    the candidates 1 .. M-1 of train.dns_candidates are then drawn in proportion to (deg_i + 1)^beta (``pop_tables``), and the
-    sampled softmax loss takes the logQ correction.  Absent or null (the default) is the uniform draw.  Raises ValueError for any
-    other value."""
-    from .config import configs
-    b = configs.get('train', {}).get('neg_popularity')
-    if b is None:
-        return None
-    if isinstance(b, bool) or not isinstance(b, (int, float)) or not 0.0 <= b <= 1.0:
-        raise ValueError(f'train.neg_popularity must be a number in [0, 1] or null, got {b!r}')
-    return float(b)
-
 
 def pop_tables(indptr, indices, n_item: int, beta: float) -> dict:
     """The host tables of the popularity draw (include/sslrec_b200.h, a27) from a training CSR with sorted, distinct columns per
@@ -1613,16 +1668,6 @@ def hard_negatives(users, items, ancs, cands: torch.Tensor) -> torch.Tensor:
 # ---- MixGCF negatives (optional key train.mixgcf) ----------------------------------------------------------------------------
 
 MIXGCF_MAX_LAYERS = 8
-
-
-def mixgcf() -> bool:
-    """The optional key ``train.mixgcf`` (INTEGRATION §2): True replaces the BPR term's negative by MixGCF's mixed negative
-    (``mixgcf_bpr_sum``); False (the default) is the plain step.  Raises ValueError for a value that is not a bool."""
-    from .config import configs
-    on = configs.get('train', {}).get('mixgcf', False)
-    if not isinstance(on, bool):
-        raise ValueError(f'train.mixgcf must be true or false, got {on!r}')
-    return on
 
 
 def _mix_grad_target(op, plain_grads: dict):
@@ -1774,19 +1819,6 @@ def _mix_operands(tables):
 
 
 # ---- sampled softmax loss (optional key train.ssm_temperature) ---------------------------------------------------------------
-
-def ssm_temperature() -> Optional[float]:
-    """The optional key ``train.ssm_temperature`` (INTEGRATION §2): tau, a finite number > 0 (int or float, not a bool), replaces
-    the BPR term by the sampled softmax loss on cosine scores over tau (``ssm_loss_sum``); absent or null (the default) is the
-    plain step.  Raises ValueError for any other value, or one that is not finite and > 0 in fp32."""
-    from .config import configs
-    t = configs.get('train', {}).get('ssm_temperature')
-    if t is None:
-        return None
-    if isinstance(t, bool) or not isinstance(t, (int, float)) or not (0.0 < C.c_float(t).value < math.inf):
-        raise ValueError(f'train.ssm_temperature must be a finite number > 0 or null, got {t!r}')
-    return float(t)
-
 
 class _SsmFn(torch.autograd.Function):
     """The sampled softmax term (``ssl_ssm_fwd`` / ``_bwd``).  Operands as in ``_MixgcfFn``: Rows (gradients into their sinks,

@@ -66,7 +66,7 @@ class HCCF(BaseModel):
             hyper_out.append(E.hyper_layer(layers[-1], a_u, a_i, self.hgnn_layer.slope,                # :48-49
                                            self._hyper_drop(keep_rate, k, 0, drop_seed), self._hyper_drop(keep_rate, k, 1, drop_seed)))
             layers.append(gcn_out[-1] + hyper_out[-1])                                         # :52
-        self._mix_tables = layers if self.mixgcf else None         # train.mixgcf mixes the item rows of every layer
+        self._mix_tables = layers if self.neg.mixgcf else None     # train.mixgcf mixes the item rows of every layer
         return sum(layers), gcn_out, hyper_out
 
     def _contrast(self, gcn_out, hyper_out, ancs, poss):
@@ -91,10 +91,10 @@ class HCCF(BaseModel):
         ancs, poss, negs = batch_data
         embeds, gcn_out, hyper_out = self.forward(self.adj, self.keep_rate)
         users, items = embeds[:self.user_num], embeds[self.user_num:]
-        cands = self._dns_candidates(ancs, negs)
+        draw = self._dns_candidates(ancs, negs)
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (hccf.py:70-74)
         layers = lambda: [t[self.user_num:] for t in self._mix_tables]
-        bpr_loss = self._bpr_term(users, items, layers, ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
+        bpr_loss = self._bpr_term(users, items, layers, ancs, poss, negs, draw, cal_bpr_loss)[0] / ancs.shape[0]
         terms = {self.bpr_loss_name: bpr_loss,
                  'reg_loss': reg_params(self) * self.reg_weight,
                  'cl_loss': self._contrast(gcn_out, hyper_out, ancs, poss) * self.cl_weight}

@@ -127,7 +127,7 @@ class LightGCL(BaseModel):
             g_i.append(v_mul_s @ (ut @ prev[:nu]))                           # :81-82
             e_list.append(z)                                                 # :86-87 (no residual)
         e = sum(e_list)
-        self._mix_tables = e_list if self.mixgcf else None         # train.mixgcf mixes the item rows of every layer
+        self._mix_tables = e_list if self.neg.mixgcf else None     # train.mixgcf mixes the item rows of every layer
         self.G_u, self.G_i = sum(g_u), sum(g_i)
         self.E_u, self.E_i = e[:nu], e[nu:]
         return self.E_u, self.E_i
@@ -136,10 +136,10 @@ class LightGCL(BaseModel):
         self.is_training = True
         user_embeds, item_embeds = self.forward()
         ancs, poss, negs = batch_data
-        cands = self._dns_candidates(ancs, negs)
+        draw = self._dns_candidates(ancs, negs)
         # -log sigmoid(a.p - a.n).mean() == softplus(a.n - a.p).mean()  (lightgcl.py:101-106)
         layers = lambda: [t[self.user_num:] for t in self._mix_tables]
-        bpr_loss = self._bpr_term(user_embeds, item_embeds, layers, ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
+        bpr_loss = self._bpr_term(user_embeds, item_embeds, layers, ancs, poss, negs, draw, cal_bpr_loss)[0] / ancs.shape[0]
         at = E.rows_at          # table[ids]; under train.deterministic with an ordered backward
         g_u, g_i = at(self.G_u, ancs), at(self.G_i, poss)
         neg_score = E.dense_logsumexp_mean(g_u, user_embeds, self.temp, 1e-8) + E.dense_logsumexp_mean(g_i, item_embeds, self.temp, 1e-8)

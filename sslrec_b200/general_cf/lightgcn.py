@@ -42,7 +42,7 @@ class LightGCN(BaseModel):
 
     def _mix_keep(self):
         """Layers the propagation keeps for train.mixgcf: 1 .. L (their item rows are mixed); none without the key."""
-        return tuple(range(1, self.layer_num + 1)) if self.mixgcf else ()
+        return tuple(range(1, self.layer_num + 1)) if self.neg.mixgcf else ()
 
     def _mix_layers(self, st, v):
         """The item rows of layers 0 .. L of view ``v`` (layer 0 = E0), for ``_bpr_term``."""
@@ -66,8 +66,8 @@ class LightGCN(BaseModel):
         ancs, poss, negs = batch_data
         st = self._propagate([self._edge_view(self.keep_rate)], keep_layers=self._mix_keep())
         self.final_embeds = st.E.view(st.n, st.dim)
-        cands = self._dns_candidates(ancs, negs)
-        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / ancs.shape[0]
+        draw = self._dns_candidates(ancs, negs)
+        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, draw, cal_bpr_loss)[0] / ancs.shape[0]
         reg_loss = self.reg_weight * reg_params(self)
         loss = bpr_loss + reg_loss
         losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss}

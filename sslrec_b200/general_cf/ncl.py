@@ -82,7 +82,7 @@ class NCL(LightGCN):
         if not getattr(self, '_graph_mode', False) and (not hasattr(self, 'user2cluster') or bool(torch.sum(kmeans_flags) != 0)):
             self._cluster()
         embeds, st = self.forward(self.adj)
-        cands = self._dns_candidates(ancs, negs)
+        draw = self._dns_candidates(ancs, negs)
         ctx = self.high_order * 2
         bsz = ancs.shape[0]
         # structure loss (ncl.py:51-58): context (layer 2*high_order) vs ego (layer 0), all ego rows as negatives
@@ -94,7 +94,7 @@ class NCL(LightGCN):
                       + cal_infonce_loss(st.items(0, 0), ic, ic, self.temperature, idx=poss, idx2=self.item2cluster[poss])) / bsz
         struct_loss = struct_loss * self.struct_weight
         proto_loss = proto_loss * self.proto_weight
-        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, cands, cal_bpr_loss)[0] / bsz
+        bpr_loss = self._bpr_term(st.users(0), st.items(0), self._mix_layers(st, 0), ancs, poss, negs, draw, cal_bpr_loss)[0] / bsz
         reg_loss = reg_params(self) * self.reg_weight
         loss = bpr_loss + struct_loss + proto_loss + reg_loss
         losses = {self.bpr_loss_name: bpr_loss, 'reg_loss': reg_loss, 'struct_loss': struct_loss, 'proto_loss': proto_loss}

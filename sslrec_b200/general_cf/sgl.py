@@ -44,14 +44,14 @@ class SGL(LightGCN):
         # anchors); view 2 becomes final_embeds and view 1 is the InfoNCE table, so both are computed at every row.  With
         # train.dns_candidates the idx=negs term reads view 0 at the selected negatives, so every candidate is a batch row
         v0, v1 = self._aug_view(keep_rate, 0), self._aug_view(keep_rate, 1)
-        cands = self._dns_candidates(ancs, negs)
-        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
+        draw = self._dns_candidates(ancs, negs)
+        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if draw is None else [(draw.cands.view(-1), self.user_num)])
         v0.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
         st = self._propagate([v0, v1, E.ViewSpec()], n_layers=configs['model']['layer_num'], keep_layers=self._mix_keep())
         self.final_embeds = st.E[:, 2, :]
         bsz = ancs.shape[0]
         # with train.mixgcf or train.ssm_temperature the idx=negs term below keeps the loader's negatives
-        bpr_loss, negs = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, cands, cal_bpr_loss)
+        bpr_loss, negs = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, draw, cal_bpr_loss)
         bpr_loss = bpr_loss / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \
             cal_infonce_loss(st.items(0), st.items(1), st.items(1), self.temperature, idx=poss) + \

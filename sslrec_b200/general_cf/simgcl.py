@@ -35,12 +35,12 @@ class SimGCL(LightGCN):
         # read at the batch rows only, so the last layer computes them there; view 1 is the InfoNCE table (every row).  With
         # train.dns_candidates the BPR term's negative is chosen on view 2 among the candidates, so they are batch rows too
         v0, v1, v2 = self._noise_view(0), self._noise_view(1), E.ViewSpec()
-        cands = self._dns_candidates(ancs, negs)
-        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if cands is None else [(cands.view(-1), self.user_num)])
+        draw = self._dns_candidates(ancs, negs)
+        rows = [(ancs, 0), (poss, self.user_num), (negs, self.user_num)] + ([] if draw is None else [(draw.cands.view(-1), self.user_num)])
         v0.row_bits = v2.row_bits = E.row_bitmap(self.user_num + self.item_num, self.user_embeds.device, *rows)
         st = self._propagate([v0, v1, v2], noise_eps=self.eps, keep_layers=self._mix_keep())
         bsz = ancs.shape[0]
-        bpr_loss = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, cands, cal_bpr_loss)[0] / bsz
+        bpr_loss = self._bpr_term(st.users(2), st.items(2), self._mix_layers(st, 2), ancs, poss, negs, draw, cal_bpr_loss)[0] / bsz
         cl_loss = cal_infonce_loss(st.users(0), st.users(1), st.users(1), self.temperature, idx=ancs) + \
             cal_infonce_loss(st.items(0), st.items(1), st.items(1), self.temperature, idx=poss)
         cl_loss = cl_loss / bsz

@@ -103,14 +103,8 @@ class Trainer(object):
         self.data_handler = data_handler
         self.logger = logger
         self.grad_sync = grad_sync     # parallel.BatchShard: data-parallel ranks average gradients before the step
-        if grad_sync is not None and E.dns_candidates() > 1:
-            raise ValueError('train.dns_candidates is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
-        if grad_sync is not None and E.mixgcf():
-            raise ValueError('train.mixgcf is single-GPU: data-parallel ranks share the seed, so their mixing weights would coincide')
-        if grad_sync is not None and E.ssm_temperature() is not None:
-            raise ValueError('train.ssm_temperature is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
-        if grad_sync is not None and E.neg_popularity() is not None:
-            raise ValueError('train.neg_popularity is single-GPU: data-parallel ranks share the seed, so their candidate draws would coincide')
+        if grad_sync is not None:
+            E.NegSpec.from_config().refuse_multi_gpu(sharded=False)
         self._graphed = None           # graphed.GraphedStep when train.cuda_graph is set
         self._writer = None            # created on first use: the scalars 'Loss/train' and 'HR/test' of trainer.py:78,144
         self.epoch_done = -1           # the last epoch train_epoch finished (a training checkpoint resumes after it)
@@ -322,14 +316,7 @@ class Trainer(object):
         record = {'model': configs['model']['name'], 'data': configs['data']['name'], 'user_num': int(model.user_num),
                   'item_num': int(model.item_num), 'model_config': deepcopy(configs['model']), 'optimizer_config': deepcopy(configs['optimizer']),
                   'batch_size': t['batch_size'], 'seed': t.get('seed'), 'loader': kind, 'deterministic': E.deterministic()}
-        if E.dns_candidates() > 1:          # only then: the records of runs without the key stay as they were
-            record['dns_candidates'] = E.dns_candidates()
-        if E.mixgcf():
-            record['mixgcf'] = True
-        if E.ssm_temperature() is not None:
-            record['ssm_temperature'] = E.ssm_temperature()
-        if E.neg_popularity() is not None:
-            record['neg_popularity'] = E.neg_popularity()
+        record.update(E.NegSpec.from_config().record())
         return record
 
     def save_checkpoint(self, model, path):

@@ -1,18 +1,13 @@
 """Dynamic negative sampling (train.dns_candidates) without a GPU: the numpy restatement of ssl_neg_candidates's draws
-(tests/dns_oracle.neg_candidates) against a scalar restatement of the documented rule, its 64-block cap, the float64 selection of
-the oracle, and the key's validation and refusals: values outside [1, 256], DirectAU, a row-sharded model, data-parallel
-gradient sync, and training checkpoints of runs with another M."""
-import types
-
+(tests/dns_oracle.neg_candidates) against a scalar restatement of the documented rule, its 64-block cap and the float64
+selection of the oracle (the key itself: tests/test_host_neg_spec.py)."""
 import numpy as np
-import pytest
 import scipy.sparse as sp
 import torch
 
 import dns_oracle as D
 from oracle import inputs
 from oracle import philox as P
-from test_host_resume import make_run
 
 
 def _csr(rows, cols, n_user, n_item):
@@ -68,53 +63,3 @@ def test_oracle_selection_ties_and_nan():
     ancs = torch.tensor([0, 0, 0])
     cands = torch.tensor([[0, 1, 2], [3, 2, 1], [3, 3, 3]])
     assert D.hard_negatives(u, items, ancs, cands).tolist() == [1, 2, 3]       # tie to the lowest j; NaN skipped; all NaN -> j = 0
-
-
-@pytest.mark.parametrize('value', [0, 257, -3, 2.5, True, '8', None])
-def test_bad_values_are_refused_at_construction(value):
-    with pytest.raises(ValueError, match='dns_candidates'):
-        make_run('lightgcn', train=dict(dns_candidates=value))
-
-
-@pytest.mark.parametrize('key', ['lightgcn', 'simgcl', 'sgl', 'ncl', 'hccf', 'lightgcl'])
-def test_every_bpr_model_accepts_the_key(key):
-    m, _, _ = make_run(key, train=dict(dns_candidates=256))
-    assert m.dns_candidates == 256 and m.dns_negs is None
-    assert make_run(key)[0].dns_candidates == 1
-
-
-def test_directau_is_refused():
-    assert make_run('directau', train=dict(dns_candidates=1))[0].dns_candidates == 1
-    with pytest.raises(ValueError, match='DirectAU trains without negatives'):
-        make_run('directau', train=dict(dns_candidates=2))
-
-
-def test_multi_gpu_is_refused():
-    from sslrec_b200.trainer import Trainer
-    m, _, dh = make_run('simgcl', train=dict(dns_candidates=8))
-    with pytest.raises(ValueError, match='single-GPU'):
-        m.shard_to(types.SimpleNamespace(shard_propagation=False))
-    assert m.comm is None
-    with pytest.raises(ValueError, match='single-GPU'):
-        Trainer(dh, grad_sync=object())
-    m, _, dh = make_run('simgcl')
-    Trainer(dh, grad_sync=object())             # without the key nothing changes
-
-
-def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
-    plain, dns = str(tmp_path / 'plain.pth'), str(tmp_path / 'dns.pth')
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
-    assert tr._resume_record(m, 'host')['dns_candidates'] == 8
-    tr.save_checkpoint(m, dns)
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=1))
-    assert 'dns_candidates' not in tr._resume_record(m, 'host')
-    tr.save_checkpoint(m, plain)
-    with pytest.raises(ValueError, match='dns_candidates: saved 8, now None'):
-        tr.load_checkpoint(m, dns)
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=4))
-    with pytest.raises(ValueError, match='dns_candidates: saved None, now 4'):
-        tr.load_checkpoint(m, plain)
-    with pytest.raises(ValueError, match='dns_candidates: saved 8, now 4'):
-        tr.load_checkpoint(m, dns)
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
-    assert tr.load_checkpoint(m, dns) == 0

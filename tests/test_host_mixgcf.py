@@ -1,11 +1,8 @@
 """MixGCF negatives (train.mixgcf) without a GPU: the numpy restatement of ssl_mixgcf_bpr_fwd's mixing weights
 (tests/mixgcf_oracle.alpha) against a scalar restatement of the documented draw, the float64 picks and term of the oracle on
-a hand-made case, the key's validation and refusals (a value that is not a bool, DirectAU, more than 8 layers, a row-sharded
-model, data-parallel gradient sync) and the training checkpoint's record of the key.  On every whole-step case of
-tests/test_gpu_mixgcf.py, on host draws: the float32 oracle meets the GPU test's bounds against float64, and three slightly
+a hand-made case, and the refusal of more than 8 layers (the key itself: tests/test_host_neg_spec.py).  On every whole-step
+case of tests/test_gpu_mixgcf.py, on host draws: the float32 oracle meets the GPU test's bounds against float64, and three slightly
 wrong MixGCF terms (layers 1 .. L reversed, each layer's gradient routed one layer deeper, the positive's share detached) do not."""
-import types
-
 import numpy as np
 import pytest
 import torch
@@ -15,8 +12,6 @@ import mixgcf_oracle as X
 import ssl_test_helpers as H
 from oracle import philox as P
 from test_host_resume import make_run
-
-BPR_MODELS = ['lightgcn', 'simgcl', 'sgl', 'ncl', 'hccf', 'lightgcl']
 
 
 def test_alpha_oracle_matches_a_scalar_restatement():
@@ -50,63 +45,11 @@ def test_oracle_picks_and_term_on_a_hand_made_case():
     assert abs(float(X.term(users.double(), items.double(), [x.double() for x in layers], ancs, poss, got, a)) - want) < 1e-12
 
 
-@pytest.mark.parametrize('value', [1, 0, 'true', None, 2.5])
-def test_bad_values_are_refused_at_construction(value):
-    with pytest.raises(ValueError, match='train.mixgcf must be true or false'):
-        make_run('lightgcn', train=dict(mixgcf=value))
-
-
-@pytest.mark.parametrize('key', BPR_MODELS)
-def test_every_bpr_model_accepts_the_key(key):
-    m, _, _ = make_run(key, train=dict(mixgcf=True, dns_candidates=8))
-    assert m.mixgcf and m.mixgcf_picks is None and m.mixgcf_alpha is None and m.dns_negs is None
-    assert not make_run(key)[0].mixgcf
-    assert not make_run(key, train=dict(mixgcf=False))[0].mixgcf
-
-
-def test_directau_is_refused():
-    assert not make_run('directau', train=dict(mixgcf=False))[0].mixgcf
-    with pytest.raises(ValueError, match='train.mixgcf: DirectAU trains without negatives'):
-        make_run('directau', train=dict(mixgcf=True))
-
-
 def test_more_than_eight_layers_are_refused():
     assert make_run('lightgcn', train=dict(mixgcf=True), model=dict(layer_num=7))[0].mixgcf
     with pytest.raises(ValueError, match='at most 8 layers'):
         make_run('lightgcn', train=dict(mixgcf=True), model=dict(layer_num=8))
     assert not make_run('lightgcn', model=dict(layer_num=8))[0].mixgcf     # without the key nothing changes
-
-
-def test_multi_gpu_is_refused():
-    from sslrec_b200.trainer import Trainer
-    m, _, dh = make_run('simgcl', train=dict(mixgcf=True))
-    with pytest.raises(ValueError, match='train.mixgcf is single-GPU'):
-        m.shard_to(types.SimpleNamespace(shard_propagation=False))
-    assert m.comm is None
-    with pytest.raises(ValueError, match='train.mixgcf is single-GPU'):
-        Trainer(dh, grad_sync=object())
-    m, _, dh = make_run('simgcl', train=dict(mixgcf=False))
-    Trainer(dh, grad_sync=object())             # without the key nothing changes
-
-
-def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
-    plain, mixed = str(tmp_path / 'plain.pth'), str(tmp_path / 'mixed.pth')
-    m, tr, _ = make_run('ncl', train=dict(mixgcf=True, dns_candidates=8))
-    rec = tr._resume_record(m, 'host')
-    assert rec['mixgcf'] is True and rec['dns_candidates'] == 8
-    tr.save_checkpoint(m, mixed)
-    m, tr, _ = make_run('ncl', train=dict(mixgcf=False, dns_candidates=8))
-    assert 'mixgcf' not in tr._resume_record(m, 'host')
-    tr.save_checkpoint(m, plain)
-    with pytest.raises(ValueError, match='mixgcf: saved True, now None'):
-        tr.load_checkpoint(m, mixed)
-    m, tr, _ = make_run('ncl', train=dict(mixgcf=True, dns_candidates=8))
-    with pytest.raises(ValueError, match='mixgcf: saved None, now True'):
-        tr.load_checkpoint(m, plain)
-    assert tr.load_checkpoint(m, mixed) == 0
-    # a record of a run without either key is what it was before the key existed
-    m, tr, _ = make_run('ncl')
-    assert not {'mixgcf', 'dns_candidates'} & set(tr._resume_record(m, 'host'))
 
 
 # ---- whole-step cases of tests/test_gpu_mixgcf.py::test_whole_step_against_float64, on host draws ------------------------------

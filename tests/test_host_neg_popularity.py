@@ -1,21 +1,20 @@
 """Popularity-proportional candidates (train.neg_popularity) without a GPU.
 
-The key's validation and refusals (a value that is not a number in [0, 1], train.dns_candidates below 2, DirectAU, a row-sharded
-model, data-parallel gradient sync) and the training checkpoint's record of the key.  The host tables of engine.pop_tables: the
-integer weights sum to n_item 2^32 exactly and the shares the alias table realises, recomputed from {thr, alias} in integers,
-equal them exactly; beta = 0 is uniform with every column self-aliased; Zipf-skewed degrees, items of degree 0, n_item = 1; the
-same table on every call; the per-user tables, a user who has every item included.  The numpy draw oracle (tests/pop_oracle)
-against a scalar restatement of the documented rule and its cap.  The draw kernel and the logQ forward of csrc/ssm.cuh run on the
-host under AddressSanitizer (tests/emu/pop_negs_emu.cpp) and equal the oracle and the float32 restatement bit for bit; with
-bias = 0 the logQ forward equals ssm_fwd_kernel bit for bit.  On every whole-step case of tests/test_gpu_neg_popularity.py, on
-host draws: the fp32 bias is within pop_oracle.bias_tol of bias64 (beta 0, 0.75 and 1); the float32 oracle with it meets the GPU
-test's bounds against the float64 oracle with bias64, and five wrong corrections (none, column 0 corrected as a popularity
-draw, lz_pop = 0, the bias of permuted anchors, tables of beta 0.7) do not."""
+The refusals of train.dns_candidates below 2 and of data-parallel gradient sync when train.dns_candidates is 1 (the key itself:
+tests/test_host_neg_spec.py).  The host tables of engine.pop_tables: the integer weights sum to n_item 2^32 exactly and the
+shares the alias table realises, recomputed from {thr, alias} in integers, equal them exactly; beta = 0 is uniform with every
+column self-aliased; Zipf-skewed degrees, items of degree 0, n_item = 1; the same table on every call; the per-user tables, a
+user who has every item included.  The numpy draw oracle (tests/pop_oracle) against a scalar restatement of the documented rule
+and its cap.  The draw kernel and the logQ forward of csrc/ssm.cuh run on the host under AddressSanitizer
+(tests/emu/pop_negs_emu.cpp) and equal the oracle and the float32 restatement bit for bit; with bias = 0 the logQ forward
+equals ssm_fwd_kernel bit for bit.  On every whole-step case of tests/test_gpu_neg_popularity.py, on host draws: the fp32 bias
+is within pop_oracle.bias_tol of bias64 (beta 0, 0.75 and 1); the float32 oracle with it meets the GPU test's bounds against
+the float64 oracle with bias64, and five wrong corrections (none, column 0 corrected as a popularity draw, lz_pop = 0, the bias
+of permuted anchors, tables of beta 0.7) do not."""
 import math
 import os
 import shutil
 import subprocess
-import types
 
 import numpy as np
 import pytest
@@ -31,48 +30,16 @@ from sslrec_b200 import engine as E
 from test_host_resume import make_run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BPR_MODELS = ['lightgcn', 'simgcl', 'sgl', 'ncl', 'hccf', 'lightgcl']
 K = 1 << 32
 
 
 # ---- the key ---------------------------------------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize('value', [True, False, -0.1, 1.5, 2, -1, float('inf'), float('nan'), '0.5', [0.5]])
-def test_bad_values_are_refused_at_construction(value):
-    with pytest.raises(ValueError, match=r'train.neg_popularity must be a number in \[0, 1\] or null'):
-        make_run('lightgcn', train=dict(neg_popularity=value, dns_candidates=8))
-
-
-@pytest.mark.parametrize('key', BPR_MODELS)
-def test_every_bpr_model_accepts_the_key(key):
-    for beta in (0, 1, 0.75):
-        m = make_run(key, train=dict(neg_popularity=beta, dns_candidates=8))[0]
-        assert m.neg_popularity == float(beta) and m._pop is None
-    for train in ({}, dict(neg_popularity=None), dict(neg_popularity=None, dns_candidates=8)):
-        assert make_run(key, train=train)[0].neg_popularity is None
-
-
-def test_one_candidate_and_directau_are_refused():
+def test_one_candidate_is_refused():
     with pytest.raises(ValueError, match='which must then be >= 2, got 1'):
         make_run('lightgcn', train=dict(neg_popularity=0.5))
     with pytest.raises(ValueError, match='which must then be >= 2, got 1'):
         make_run('lightgcn', train=dict(neg_popularity=0.5, ssm_temperature=0.1))
-    assert make_run('directau', train=dict(neg_popularity=None))[0].neg_popularity is None
-    with pytest.raises(ValueError, match='train.neg_popularity: DirectAU trains without negatives'):
-        make_run('directau', train=dict(neg_popularity=0.5))
-
-
-def test_multi_gpu_is_refused():
-    from sslrec_b200.trainer import Trainer
-    m, _, dh = make_run('simgcl', train=dict(neg_popularity=0.5, dns_candidates=8))
-    m.dns_candidates = 1                       # the draw key alone must refuse the row-sharded model
-    with pytest.raises(ValueError, match='train.neg_popularity is single-GPU'):
-        m.shard_to(types.SimpleNamespace(shard_propagation=False))
-    assert m.comm is None
-    with pytest.raises(ValueError, match='single-GPU'):
-        Trainer(dh, grad_sync=object())
-    _, _, dh = make_run('simgcl', train=dict(neg_popularity=None, dns_candidates=1))
-    Trainer(dh, grad_sync=object())             # without the key nothing changes
 
 
 def test_grad_sync_names_the_key():
@@ -82,26 +49,6 @@ def test_grad_sync_names_the_key():
     config.configs['train']['dns_candidates'] = 1          # the earlier refusal would name train.dns_candidates
     with pytest.raises(ValueError, match='train.neg_popularity is single-GPU'):
         Trainer(dh, grad_sync=object())
-
-
-def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
-    a, plain = str(tmp_path / 'a.pth'), str(tmp_path / 'plain.pth')
-    m, tr, _ = make_run('ncl', train=dict(neg_popularity=0.5, dns_candidates=8))
-    assert tr._resume_record(m, 'host')['neg_popularity'] == 0.5
-    tr.save_checkpoint(m, a)
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
-    assert 'neg_popularity' not in tr._resume_record(m, 'host')
-    tr.save_checkpoint(m, plain)
-    with pytest.raises(ValueError, match='neg_popularity: saved 0.5, now None'):
-        tr.load_checkpoint(m, a)
-    m, tr, _ = make_run('ncl', train=dict(neg_popularity=0.75, dns_candidates=8))
-    with pytest.raises(ValueError, match='neg_popularity: saved 0.5, now 0.75'):
-        tr.load_checkpoint(m, a)
-    with pytest.raises(ValueError, match='neg_popularity: saved None, now 0.75'):
-        tr.load_checkpoint(m, plain)
-    m, tr, _ = make_run('ncl', train=dict(neg_popularity=0.5, dns_candidates=8))
-    assert tr.load_checkpoint(m, a) == 0
-    assert m._pop is None                       # the tables are not part of a checkpoint
 
 
 # ---- the host tables ---------------------------------------------------------------------------------------------------------

@@ -1,10 +1,7 @@
-"""The sampled softmax loss (train.ssm_temperature) without a GPU: the key's validation and refusals (a value that is not a
-finite number > 0, the key together with train.mixgcf, DirectAU, a row-sharded model, data-parallel gradient sync), the
-training checkpoint's record of the key, and the oracle's identities (M = 1 is softplus(s_0' - s_+); the fp32 restatement
+"""The sampled softmax loss (train.ssm_temperature) without a GPU: the refusal of the key together with train.mixgcf (the key
+itself: tests/test_host_neg_spec.py), and the oracle's identities (M = 1 is softplus(s_0' - s_+); the fp32 restatement
 against float64).  On every whole-step case of tests/test_gpu_ssm.py, on host draws: the float32 oracle meets the GPU test's
 bounds against float64, and one at tau (1 + 1e-3) does not."""
-import types
-
 import numpy as np
 import pytest
 import torch
@@ -15,68 +12,11 @@ import ssl_test_helpers as H
 import ssm_oracle as S
 from test_host_resume import make_run
 
-BPR_MODELS = ['lightgcn', 'simgcl', 'sgl', 'ncl', 'hccf', 'lightgcl']
-
-
-@pytest.mark.parametrize('value', [True, False, 0, 0.0, -0.5, -2, float('inf'), float('nan'), '0.1', [0.1], 1e-50, 1e39])
-def test_bad_values_are_refused_at_construction(value):
-    with pytest.raises(ValueError, match='train.ssm_temperature must be a finite number > 0 or null'):
-        make_run('lightgcn', train=dict(ssm_temperature=value))
-
-
-@pytest.mark.parametrize('key', BPR_MODELS)
-def test_every_bpr_model_accepts_the_key(key):
-    m, _, _ = make_run(key, train=dict(ssm_temperature=0.1, dns_candidates=8))
-    assert m.ssm_temperature == 0.1 and m.bpr_loss_name == 'ssm_loss' and m.dns_negs is None
-    assert make_run(key, train=dict(ssm_temperature=2))[0].ssm_temperature == 2.0          # an int is a number
-    for train in ({}, dict(ssm_temperature=None)):
-        m = make_run(key, train=train)[0]
-        assert m.ssm_temperature is None and m.bpr_loss_name == 'bpr_loss'
-
 
 def test_mixgcf_is_refused():
     with pytest.raises(ValueError, match='train.ssm_temperature and train.mixgcf both replace the BPR term'):
         make_run('lightgcn', train=dict(ssm_temperature=0.1, mixgcf=True))
     assert make_run('lightgcn', train=dict(ssm_temperature=0.1, mixgcf=False))[0].ssm_temperature == 0.1
-
-
-def test_directau_is_refused():
-    assert make_run('directau', train=dict(ssm_temperature=None))[0].ssm_temperature is None
-    with pytest.raises(ValueError, match='train.ssm_temperature: DirectAU trains without negatives'):
-        make_run('directau', train=dict(ssm_temperature=0.1))
-
-
-def test_multi_gpu_is_refused():
-    from sslrec_b200.trainer import Trainer
-    m, _, dh = make_run('simgcl', train=dict(ssm_temperature=0.1))
-    with pytest.raises(ValueError, match='train.ssm_temperature is single-GPU'):
-        m.shard_to(types.SimpleNamespace(shard_propagation=False))
-    assert m.comm is None
-    with pytest.raises(ValueError, match='train.ssm_temperature is single-GPU'):
-        Trainer(dh, grad_sync=object())
-    m, _, dh = make_run('simgcl', train=dict(ssm_temperature=None))
-    Trainer(dh, grad_sync=object())             # without the key nothing changes
-
-
-def test_checkpoints_record_the_key_only_when_it_is_set(tmp_path):
-    a, b, plain = str(tmp_path / 'a.pth'), str(tmp_path / 'b.pth'), str(tmp_path / 'plain.pth')
-    m, tr, _ = make_run('ncl', train=dict(ssm_temperature=0.1, dns_candidates=8))
-    rec = tr._resume_record(m, 'host')
-    assert rec['ssm_temperature'] == 0.1 and rec['dns_candidates'] == 8
-    tr.save_checkpoint(m, a)
-    m, tr, _ = make_run('ncl', train=dict(ssm_temperature=0.2, dns_candidates=8))
-    tr.save_checkpoint(m, b)
-    with pytest.raises(ValueError, match='ssm_temperature: saved 0.1, now 0.2'):
-        tr.load_checkpoint(m, a)
-    m, tr, _ = make_run('ncl', train=dict(dns_candidates=8))
-    assert 'ssm_temperature' not in tr._resume_record(m, 'host')
-    tr.save_checkpoint(m, plain)
-    with pytest.raises(ValueError, match='ssm_temperature: saved 0.1, now None'):
-        tr.load_checkpoint(m, a)
-    m, tr, _ = make_run('ncl', train=dict(ssm_temperature=0.1, dns_candidates=8))
-    with pytest.raises(ValueError, match='ssm_temperature: saved None, now 0.1'):
-        tr.load_checkpoint(m, plain)
-    assert tr.load_checkpoint(m, a) == 0
 
 
 def _case(B, M, d, seed=0):

@@ -110,7 +110,7 @@ def launch_record(workload, L, dev):
         model.cal_loss(batch)[0].backward()
         st = model._state
         ancs, poss = batch[0], batch[1]
-        cands = model._dns_candidates(ancs, batch[2])
+        cands = model._dns_candidates(ancs, batch[2]).cands
         users, items = st.users(view), st.items(view)
         layers = [st.items(view, k) for k in range(model.layer_num + 1)]
 

@@ -68,7 +68,7 @@ def launch_record(workload, L, dev):
         model.cal_loss(batch)[0].backward()
         st = model._state
         ancs, poss = batch[0], batch[1]
-        cands = model._dns_candidates(ancs, batch[2])
+        cands = model._dns_candidates(ancs, batch[2]).cands
         u_ptr, u_stride, d = E._score_table(st.users(view))
         i_ptr, i_stride, _ = E._score_table(st.items(view))
         B = ancs.numel()
