@@ -601,6 +601,44 @@ SSL_API int ssl_ssm_fwd_logq(const float *u_tbl, int64_t u_stride, const float *
                              const int64_t *poss, const int64_t *cands, int64_t n_pairs, int32_t M, int32_t dim, float tau,
                              float *loss_b, float *s, float *w, float *nrm, const float *bias, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * a28  (no counterpart: in-batch negatives for the sampled softmax, mixed negative sampling of
+ *   Yang et al. WWW 2020 with the logQ correction of Yi et al. RecSys 2019; optional key
+ *   train.ssm_in_batch with train.ssm_temperature = tau)
+ *   For every pair b with u = U[ancs[b]] and the 2B columns id_c = poss[c] (c < B), negs[c - B]
+ *   (B <= c < 2B), shared by every pair, duplicates kept, x^ = x / sqrt(1e-8 + |x|^2):
+ *     s_bc = (u^ . i^_{id_c}) / tau;   w_c = v[id_c] / B (fp32 division);
+ *     loss_b = ln(sum_c w_c exp(s_bc)) - s_bb
+ *   v [n_item] fp32 (engine.in_batch_weights, float64 then fp32 once): v_i = 1 / (p_i + r_i), 0
+ *   when p_i + r_i = 0, with p_i = deg_i / |E| and r_i = sum_u (deg_u / |E|) [i not in P_u] /
+ *   (n_item - deg_u): the probability that one positive / negative slot of the loaders holds i.
+ *   The term is the InfoNCE pieces of a13/a14, no new forward:
+ *     ssl_rows_normalize[_f16x3] (norm_mode 0) of U[ancs] scaled by log2(e) / tau and of the
+ *       columns at alpha 1, both with the copies of either role; rows 0 .. B-1 of the column
+ *       operand are the positives' p^;
+ *     the contraction of users against columns with colscale = w, offset log2(e) / tau, row sums:
+ *       rowsum_b = sum_c w_c exp(s_bc - 1/tau);
+ *     ssl_nce_finalize with deno_eps 0: loss_b = -(u^ . p^_b)/tau + 1/tau + ln(rowsum_b);
+ *     backward: ssl_nce_bwd_rows (user rows by ancs, positive rows by poss), ssl_nce_colscale,
+ *       the swapped contraction (R = columns, C = users) and ssl_nce_bwd_cols.
+ *   The 3xFP16 kernel serves the weighted forward only when its E' = exp2(S - offset) w_c 2^14 / M
+ *   (M = 2^e >= max w, so w_c / M > 2^-1 min w / max w) cannot fall below the flush threshold
+ *   2^-14: E' >= 2^(13 - 2 offset) min w / max w >= 2^-13 needs offset + (1 + log2(max w / min w)) / 2
+ *   <= 13.5 (csrc/f16x3.cuh's kF16NoFlushOffset).  Past it an E' below 2^-14 is carried by its lo
+ *   part alone, at 2^-11 relative instead of 2^-22, and a row whose sum is made of such entries
+ *   (every cosine low against popular, low-weight columns; at tau = 0.1 the offset alone is
+ *   14.4) gets its loss and softmax weights at 2^-11: not fp32 grade.  The engine then takes
+ *   3xTF32 (engine.contraction_kind, from the weight table's range, known on the host).
+ *   ssl_nce_bwd_cols: the column gradient.  For c < n (= 2B), in the fp32 order of
+ *   csrc/ssm_in_batch.cuh:  d = (sum_s dt_part[s, c]) * colw[c];
+ *     sink[ids[c]] += rinv_c (d - t^_c (t^_c . d))   (float atomics; ids NULL: row c, into a -0.0
+ *   stage whose rows train.deterministic scatters in order).  t_hat [n, dim] row-major, rinv [n],
+ *   colw [n], dt_part [n_split, n, dim].  dim <= SSL_MAX_DIM, stride >= dim, n_split >= 1; n = 0 is
+ *   a no-op; rejected arguments write nothing.
+ * ------------------------------------------------------------------------------------------ */
+SSL_API int ssl_nce_bwd_cols(const float *dt_part, int32_t n_split, const float *t_hat, const float *rinv, const float *colw,
+                             const int64_t *ids, int64_t n, int32_t dim, float *sink, int64_t stride, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

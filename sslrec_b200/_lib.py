@@ -120,6 +120,7 @@ def _load():
         'ssl_ssm_bwd': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, f32, vp, i64, vp, i64, vp]),
         'ssl_neg_candidates_pop': (C.c_int, [vp, vp, i64, i32, vp, vp, i64, vp, vp, vp, vp, f32, C.c_uint64, vp, vp, vp, vp]),
         'ssl_ssm_fwd_logq': (C.c_int, [vp, i64, vp, i64, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp, vp]),
+        'ssl_nce_bwd_cols': (C.c_int, [vp, i32, vp, vp, vp, vp, i64, i32, vp, i64, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)          # AttributeError here = the .so does not export what the header declares

@@ -101,6 +101,7 @@ class BaseModel(nn.Module):
         self.dns_negs = self.mixgcf_picks = self.mixgcf_alpha = self._mix_seed = None
         self._mix_alpha_in = None      # tests: injected [B, L+1] mixing weights instead of the seeded draw
         self._pop = None               # engine.PopTables of train.neg_popularity, built once (``_pop_tables``)
+        self._in_batch = None          # engine.InBatchWeights of train.ssm_in_batch, built once (``_in_batch_weights``)
 
     bpr_negatives = True           # the loss has a BPR term with sampled negatives (train.dns_candidates / mixgcf / ssm_temperature apply)
     # the keys of ``neg`` under their config names, read-only
@@ -108,6 +109,7 @@ class BaseModel(nn.Module):
     mixgcf = property(lambda self: self.neg.mixgcf)
     ssm_temperature = property(lambda self: self.neg.ssm_temperature)
     neg_popularity = property(lambda self: self.neg.popularity)
+    ssm_in_batch = property(lambda self: self.neg.in_batch)
 
     @property
     def bpr_loss_name(self) -> str:
@@ -120,11 +122,11 @@ class BaseModel(nn.Module):
         step draws every seed of the plain step in the same order; MixGCF keys its mixing weights by the same seed, and with
         M = 1 its candidates are the loader's negatives (no draw).  The sampled softmax loss with M = 1 takes the loader's
         negatives without drawing a seed.  With train.neg_popularity the candidates come from the popularity draw on the same seed, and
-        with the sampled softmax the draw also returns their logQ correction."""
+        with the sampled softmax the draw also returns their logQ correction.  train.ssm_in_batch draws nothing: None."""
         from . import engine as E
         neg = self.neg
         if neg.candidates == 1 and not neg.mixgcf:
-            if neg.ssm_temperature is None:
+            if neg.ssm_temperature is None or neg.in_batch:
                 return None
             seed = None
         else:
@@ -151,15 +153,30 @@ class BaseModel(nn.Module):
             self._pop = E.PopTables(m.indptr.astype(np.int64), m.indices.astype(np.int64), self.item_num, self.neg.popularity, device)
         return self._pop
 
+    def _in_batch_weights(self, device):
+        """The column weights of train.ssm_in_batch (``engine.InBatchWeights``) on ``device``, built once from the training CSR:
+        a pure function of the training matrix, so checkpoints do not store it."""
+        from . import engine as E
+        if self._in_batch is None or self._in_batch.v.device != device:
+            import numpy as np
+            import scipy.sparse as sp
+            m = sp.csr_matrix(self._trn_mat)
+            m.sort_indices()
+            self._in_batch = E.InBatchWeights.of_matrix(m.indptr.astype(np.int64), m.indices.astype(np.int64), self.item_num, device)
+        return self._in_batch
+
     def _bpr_term(self, users, items, item_layers, ancs, poss, negs, draw, bpr):
         """The batch's BPR sum and the negatives every other term of ``cal_loss`` reads: the plain term (``draw`` None); with DNS
         the term on the selected candidates of ``draw`` (which the other terms then read too); with MixGCF
         ``engine.mixgcf_bpr_sum`` and with train.ssm_temperature ``engine.ssm_loss_sum`` on them (the other terms keep the
-        loader's negatives).  ``users`` / ``items`` are the summed table as Rows or [n, d] tensors; ``item_layers()`` lists the
-        item rows of its layers 0 .. L (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the plain and DNS terms call
+        loader's negatives); with train.ssm_in_batch ``engine.ssm_in_batch_sum`` over the batch's own items.  ``users`` /
+        ``items`` are the summed table as Rows or [n, d] tensors; ``item_layers()`` lists the item rows of its layers 0 .. L
+        (called with MixGCF only).  ``bpr``: the ``cal_bpr_loss`` the plain and DNS terms call
         (a model passes its module's, so a restatement can stand in for it)."""
         from . import engine as E
         rows = isinstance(users, E.Rows)
+        if self.neg.in_batch:          # no draw: every pair against the batch's positives and loader negatives
+            return E.ssm_in_batch_sum(users, items, ancs, poss, negs, self.neg.ssm_temperature, self._in_batch_weights(ancs.device)), negs
         if draw is not None:
             if self.neg.mixgcf:
                 loss, self.mixgcf_picks, self.mixgcf_alpha = E.mixgcf_bpr_sum(users, items, item_layers(), ancs, poss, draw.cands,

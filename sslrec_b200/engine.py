@@ -35,6 +35,9 @@ USE_TENSOR_CORES = True
 # ssl_softmax_gemm_f16x3 accepts unit rows scaled by |alpha| <= 16 and offsets in [0, 16] (csrc/f16x3.cuh): every InfoNCE
 # temperature >= 0.0902 and the uniformity term.  Raw rows (LightGCL) and larger offsets keep the 3xTF32 kernel.
 F16X3_MAX_OFFSET = 16.0
+# a forward with column weights (ssm_in_batch_sum) keeps 3xFP16 only while no E' can fall below the flush threshold: up to this
+# offset plus half the binades of its weights' range (csrc/f16x3.cuh's kF16NoFlushOffset; include/sslrec_b200.h, a28)
+F16X3_NO_FLUSH_OFFSET = 13.5
 LIVE_ROWS, LIVE_COLS = 1, 2     # SSL_LIVE_ROWS / SSL_LIVE_COLS: which operand of a *_live contraction the device count bounds
 NUM_SM = 132          # H100 SXM; grids of the contraction are sized in resident-CTA slots (kNumSM in csrc/common.cuh)
 
@@ -911,12 +914,17 @@ def choose_split(n_rtiles: int, n_ctiles: int, slots: int = 2 * NUM_SM, prefer_f
     return max(effs, key=lambda t: (round(t[0], 9), -t[1]))[1]
 
 
-def contraction_kind(d: int, offset: float, raw: bool = False) -> str:
+def contraction_kind(d: int, offset: float, raw: bool = False, colscale_range: Optional[float] = None) -> str:
     """The InfoNCE contraction kernel for rows of width ``d`` at ``offset``: 'ffma' (FP32 FMA, any d), 'tf32x3' (3xTF32 on the
-    tensor cores: raw rows, which the 3xFP16 operand bound does not cover, and offsets above F16X3_MAX_OFFSET) or 'f16x3'."""
+    tensor cores: raw rows, which the 3xFP16 operand bound does not cover, and offsets above F16X3_MAX_OFFSET) or 'f16x3'.
+    ``colscale_range``: max / min of the column weights of a weighted forward (``ssm_in_batch_sum``); 3xFP16 takes it only
+    while offset + (1 + log2(range)) / 2 <= F16X3_NO_FLUSH_OFFSET, where no E' reaches the flush rule (the bound is derived in
+    include/sslrec_b200.h, a28); past it an E' below 2^-14 keeps 2^-11 of its digits, so 3xTF32 runs it."""
     if not USE_TENSOR_CORES or d not in (32, 64):
         return 'ffma'
     if raw or not f16x3_applies(offset):
+        return 'tf32x3'
+    if colscale_range is not None and offset + 0.5 * (1.0 + math.log2(colscale_range)) > F16X3_NO_FLUSH_OFFSET:
         return 'tf32x3'
     return 'f16x3'
 
@@ -975,9 +983,10 @@ _GEMM_ENTRY = dict(ffma='ssl_softmax_gemm', tf32x3='ssl_softmax_gemm_tf32x3', f1
 
 
 def _contract(R: Operand, C: Operand, colscale, offset: float, n_split: int, rowsum_part, o_part, s: int, live=None,
-              live_role: int = LIVE_ROWS):
+              live_role: int = LIVE_ROWS, bwd: Optional[bool] = None):
     """One launch of the contraction of R against C on their kernel, timed as the forward role (R = anchors) or, with
-    ``colscale``, the backward role (R = table, C = anchors).  ``live``: the device count that bounds the ``live_role`` side."""
+    ``colscale``, the backward role (R = table, C = anchors).  ``live``: the device count that bounds the ``live_role`` side.
+    ``bwd`` names the role where ``colscale`` does not tell it: the weighted forward of ``ssm_in_batch_sum`` passes False."""
     name = _GEMM_ENTRY[R.kind] + ('' if live is None else '_live')
     if R.kind == 'ffma':
         ops = (R.hat.data_ptr(), R.n, C.hat.data_ptr(), C.t.data_ptr(), C.n)
@@ -986,7 +995,7 @@ def _contract(R: Operand, C: Operand, colscale, offset: float, n_split: int, row
     else:
         ops = (R.hi.data_ptr(), R.lo.data_ptr(), R.n, C.hi.data_ptr(), C.lo.data_ptr(), C.n)
     tail = () if live is None else (live.data_ptr(), live_role)
-    d, bwd = R.hat.shape[1], colscale is not None
+    d, bwd = R.hat.shape[1], (colscale is not None) if bwd is None else bwd
     meta = dict(B=C.n, n=R.n) if bwd else dict(B=R.n, n=C.n)
     with _timed('nce_gemm_bwd' if bwd else 'nce_gemm_fwd', dict(meta, dim=d, tc=R.kind != 'ffma')):
         check(getattr(lib, name)(*ops, d, _ptr(colscale), offset, n_split, _ptr(rowsum_part), o_part.data_ptr(), *tail, s),
@@ -1454,6 +1463,8 @@ _SINGLE_GPU = {
     'mixgcf': ('a row-sharded model does not mix negatives', 'data-parallel ranks share the seed, so their mixing weights would coincide'),
     'ssm_temperature': ('a row-sharded model does not score sampled candidates', _SHARED_SEED),
     'neg_popularity': ('a row-sharded model does not draw candidates', _SHARED_SEED),
+    'ssm_in_batch': ("a row-sharded model does not contract the batch's items",
+                     'each rank would contract only its share of the batch, so N ranks would not equal one step at N times the batch'),
 }
 
 
@@ -1467,11 +1478,14 @@ class NegSpec:
     the sampled softmax loss on cosine scores over tau (``ssm_loss_sum``).
     ``popularity`` (train.neg_popularity): beta, a number in [0, 1] (int or float, not a bool); the candidates 1 .. M-1 are then
     drawn in proportion to (deg_i + 1)^beta (``pop_tables``), and the sampled softmax takes their logQ correction.
+    ``in_batch`` (train.ssm_in_batch): True scores every pair of the sampled softmax against the batch's 2B items (its
+    positives and loader negatives) with the weights of ``in_batch_weights`` instead of drawn candidates (``ssm_in_batch_sum``).
     The two numbers are None when absent or null (the default)."""
     candidates: int = 1
     mixgcf: bool = False
     ssm_temperature: Optional[float] = None
     popularity: Optional[float] = None
+    in_batch: bool = False
 
     @classmethod
     def from_config(cls) -> 'NegSpec':
@@ -1490,7 +1504,10 @@ class NegSpec:
         beta = t.get('neg_popularity')
         if beta is not None and (isinstance(beta, bool) or not isinstance(beta, (int, float)) or not 0.0 <= beta <= 1.0):
             raise ValueError(f'train.neg_popularity must be a number in [0, 1] or null, got {beta!r}')
-        return cls(m, on, None if tau is None else float(tau), None if beta is None else float(beta))
+        ib = t.get('ssm_in_batch', False)
+        if not isinstance(ib, bool):
+            raise ValueError(f'train.ssm_in_batch must be true or false, got {ib!r}')
+        return cls(m, on, None if tau is None else float(tau), None if beta is None else float(beta), ib)
 
     def record(self) -> dict:
         """The keys that are set, under their config names and in the order above: what a training checkpoint records.  A key
@@ -1504,19 +1521,21 @@ class NegSpec:
             rec['ssm_temperature'] = self.ssm_temperature
         if self.popularity is not None:
             rec['neg_popularity'] = self.popularity
+        if self.in_batch:
+            rec['ssm_in_batch'] = True
         return rec
 
     def refuse_multi_gpu(self, sharded: bool) -> None:
-        """Raise ValueError naming the first set key: every key is single-GPU, for a row-sharded model (``sharded``) and for
-        data-parallel gradient sync alike."""
-        key = next(iter(self.record()), None)
+        """Raise ValueError naming the first set key (train.ssm_in_batch before the others, whose reasons it does not share):
+        every key is single-GPU, for a row-sharded model (``sharded``) and for data-parallel gradient sync alike."""
+        key = 'ssm_in_batch' if self.in_batch else next(iter(self.record()), None)
         if key is not None:
             raise ValueError(f'train.{key} is single-GPU: {_SINGLE_GPU[key][0 if sharded else 1]}')
 
     def check_model(self, model) -> None:
         """The rules that involve the model or two keys, in this order: a model without a BPR term (``bpr_negatives`` False)
         takes none of the keys; MixGCF mixes at most MIXGCF_MAX_LAYERS layers; the sampled softmax and MixGCF both replace the
-        BPR term; the popularity draw needs M >= 2."""
+        BPR term; the popularity draw needs M >= 2; the in-batch softmax needs the sampled softmax and draws no candidates."""
         key = next(iter(self.record()), None)
         if key is not None and not model.bpr_negatives:
             raise ValueError(f'train.{key}: {type(model).__name__} trains without negatives')
@@ -1527,6 +1546,11 @@ class NegSpec:
         if self.popularity is not None and self.candidates < 2:
             raise ValueError('train.neg_popularity draws the candidates of train.dns_candidates, which must then be >= 2, '
                              f'got {self.candidates}')
+        if self.in_batch and self.ssm_temperature is None:
+            raise ValueError('train.ssm_in_batch is a form of the sampled softmax: it needs train.ssm_temperature')
+        if self.in_batch and self.candidates > 1:
+            raise ValueError("train.ssm_in_batch scores the batch's own items, so the candidates of train.dns_candidates would be "
+                             f'drawn and never read: it must be 1, got {self.candidates}')
 
 
 def neg_candidates(users, negs, m: int, trn_rowptr: torch.Tensor, trn_cols: torch.Tensor, n_item: int, seed, pop=None,
@@ -1907,6 +1931,150 @@ def ssm_loss_sum(users, items, ancs, poss, cands: torch.Tensor, temp: float, bia
     ops, plain = _mix_operands([users, items])
     pack = (ops, ancs, poss, cands, float(temp), bias, len(plain))
     return _SsmFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
+
+
+# ---- in-batch negatives for the sampled softmax (optional key train.ssm_in_batch) -------------------------------------------
+
+def in_batch_weights(indptr, indices, n_item: int) -> np.ndarray:
+    """v [n_item] float64, the column weights of the in-batch softmax (include/sslrec_b200.h, a28), from a training CSR with
+    distinct columns per row: v_i = 1 / (p_i + r_i) (0 when p_i + r_i = 0), where
+
+        p_i = deg_i / |E|                                                 a positive slot holds i (uniform over the edges)
+        r_i = sum_u (deg_u / |E|) [i not in P_u] / (n_item - deg_u)       a negative slot holds i (uniform over u's non-positives)
+
+    r_i is computed in O(|E|) as (T - sum_{u holding i} a_u) / |E|, a_u = deg_u / (n_item - deg_u) (0 for a user who holds
+    every item: no loader can serve it a negative), T = sum_u a_u.  B (p_i + r_i) is the expected count of i among the 2B
+    columns of a batch of B pairs, so sum_c v[id_c] / B f(id_c) is an unbiased estimate of sum_i f(i) over the catalogue
+    (Hansen-Hurwitz; the logQ correction of Yi et al. with the loaders' exact proposal).  It holds for the marginal law of
+    the columns: a pair's own two columns follow its user's law, and nothing corrects for that.  Columns that are training
+    positives of the pair's user are kept.  A pure function of the training matrix; ``InBatchWeights`` rounds it to fp32 once."""
+    indptr = np.asarray(indptr, dtype=np.int64)
+    indices = np.asarray(indices, dtype=np.int64)
+    n = int(n_item)
+    if n < 1:
+        raise ValueError(f'in_batch_weights: n_item {n} < 1')
+    n_edge = int(indices.size)
+    v = np.zeros(n, dtype=np.float64)
+    if n_edge == 0:
+        return v
+    deg_u = np.diff(indptr).astype(np.float64)
+    free = n - deg_u
+    a = np.where(free > 0, deg_u / np.maximum(free, 1.0), 0.0)
+    held = np.bincount(indices, weights=np.repeat(a, np.diff(indptr)), minlength=n)
+    r = np.maximum(math.fsum(a.tolist()) - held, 0.0) / n_edge
+    p = np.bincount(indices, minlength=n).astype(np.float64) / n_edge
+    q = p + r
+    np.divide(1.0, q, out=v, where=q > 0)
+    return v
+
+
+class InBatchWeights:
+    """``in_batch_weights`` on a device: ``v`` fp32 [n_item] (rounded once), and ``range``, max v / min v over the items with
+    v > 0, which bounds the weights of any batch's columns and picks the forward's kernel (``contraction_kind``) on the host."""
+
+    def __init__(self, v, device):
+        v32 = np.asarray(v).astype(np.float32)
+        live = v32[v32 > 0].astype(np.float64)
+        if v32.ndim != 1 or not np.all(np.isfinite(v32)) or live.size == 0 or (v32 < 0).any():
+            raise ValueError('in-batch weights must be a finite, non-negative [n_item] vector with a positive entry')
+        self.n_item, self.range = int(v32.size), float(live.max() / live.min())
+        self.v = torch.from_numpy(v32).to(device)
+
+    @classmethod
+    def of_matrix(cls, indptr, indices, n_item: int, device) -> 'InBatchWeights':
+        return cls(in_batch_weights(indptr, indices, n_item), device)
+
+
+def _in_batch_rows(op) -> Rows:
+    """An operand of ``_mix_operands`` as the Rows the operand builder gathers from."""
+    return op if isinstance(op, Rows) else Rows.constant(op[1])
+
+
+class _SsmInBatchFn(torch.autograd.Function):
+    """The in-batch sampled softmax (include/sslrec_b200.h, a28) on the InfoNCE contraction.  Operands as in ``_SsmFn``."""
+
+    @staticmethod
+    def forward(ctx, pack, *inputs):
+        ops, ancs, poss, negs, tau, weights, n_plain = pack
+        users, items = (_in_batch_rows(op) for op in ops)
+        d = users.dim
+        if items.dim != d:
+            raise RuntimeError('sslrec_b200: the user and item rows of an in-batch softmax term differ in width')
+        dev, B = ancs.device, ancs.numel()
+        f = dict(device=dev, dtype=torch.float32)
+        cols = torch.cat([poss, negs])
+        off = LOG2E / tau
+        kind = contraction_kind(d, off, colscale_range=weights.range)
+        rowsum, obar, loss_b, out = torch.empty(B, **f), torch.empty(B, d, **f), torch.empty(B, **f), torch.empty((), **f)
+        with torch.cuda.device(dev):
+            s = _stream(ancs)
+            # users are R here and C in the backward, the columns the other way round: both get the copies of either role
+            a = _operand(users, ancs, 0, off, s, kind, streamed=True)
+            t = _operand(items, cols, 0, 1.0, s, kind, streamed=True)
+            w = torch.zeros(t.npad, **f)              # the padded tail is read (then masked) by the tile loads
+            torch.div(weights.v.index_select(0, cols), B, out=w[:2 * B])
+            n_split = _n_split(a, t)
+            rs_part, o_part = torch.zeros(n_split, B, **f), torch.zeros(n_split, B, d, **f)
+            _contract(a, t, w, off, n_split, rs_part, o_part, s, bwd=False)
+            # rows 0 .. B-1 of the columns are the positives' p^
+            check(lib.ssl_nce_finalize(rs_part.data_ptr(), o_part.data_ptr(), n_split, B, d, a.hat.data_ptr(), t.hat.data_ptr(), tau,
+                                       0.0, rowsum.data_ptr(), obar.data_ptr(), loss_b.data_ptr(), s), 'ssl_nce_finalize')
+            check(lib.ssl_sum(loss_b.data_ptr(), B, 1.0, out.data_ptr(), s), 'ssl_sum')
+        ctx.pack = (ops, ancs, poss, cols, tau, a, t, w, rowsum, obar, n_plain, len(inputs) - n_plain)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        ops, ancs, poss, cols, tau, a, t, w, rowsum, obar, n_plain, n_tokens = ctx.pack
+        g = g.contiguous()
+        plain_grads: dict = {}
+        targets = [_mix_grad_target(op, plain_grads) for op in ops]
+        if any(p is None for p, _ in targets):
+            raise RuntimeError('sslrec_b200: every operand of an in-batch softmax term must take a gradient')
+        (gu, gu_s), (gi, gi_s) = targets
+        dev, B, d = g.device, ancs.numel(), a.hat.shape[1]
+        f = dict(device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            s = _stream(g)
+            colscale = torch.zeros(a.npad, **f)
+            check(lib.ssl_nce_colscale(rowsum.data_ptr(), B, g.data_ptr(), 1.0, colscale.data_ptr(), s), 'ssl_nce_colscale')
+            n_split = _n_split(t, a)
+            dt_part = torch.empty(n_split, 2 * B, d, **f)
+            _contract(t, a, colscale, LOG2E / tau, n_split, None, dt_part, s, bwd=True)
+            rows = (a.hat.data_ptr(), t.hat.data_ptr(), obar.data_ptr(), a.rinv.data_ptr(), t.rinv.data_ptr())
+            if deterministic():
+                # identity ids into one -0.0 stage: users (positions ancs), the positives' row term (poss), the columns (cols)
+                stage = _stage(4 * B, d, dev)
+                ar = torch.arange(B, device=dev)
+                check(lib.ssl_nce_bwd_rows(*rows, ar.data_ptr(), B, d, tau, g.data_ptr(), 1.0, stage.data_ptr(), d,
+                                           stage[B:].data_ptr(), d, s), 'ssl_nce_bwd_rows')
+                check(lib.ssl_nce_bwd_cols(dt_part.data_ptr(), n_split, t.hat.data_ptr(), t.rinv.data_ptr(), w.data_ptr(), None, 2 * B, d,
+                                           stage[2 * B:].data_ptr(), d, s), 'ssl_nce_bwd_cols')
+                _scatter_grouped([(stage[:B], ancs, gu, gu_s), (stage[B:], torch.cat([poss, cols]), gi, gi_s)])
+            else:
+                check(lib.ssl_nce_bwd_rows(*rows, ancs.data_ptr(), B, d, tau, g.data_ptr(), 1.0, gu, gu_s, None, 0, s), 'ssl_nce_bwd_rows')
+                check(lib.ssl_nce_bwd_rows(*rows, poss.data_ptr(), B, d, tau, g.data_ptr(), 1.0, None, 0, gi, gi_s, s), 'ssl_nce_bwd_rows')
+                check(lib.ssl_nce_bwd_cols(dt_part.data_ptr(), n_split, t.hat.data_ptr(), t.rinv.data_ptr(), w.data_ptr(), cols.data_ptr(),
+                                           2 * B, d, gi, gi_s, s), 'ssl_nce_bwd_cols')
+        zero = torch.zeros((), device=dev)
+        return (None,) + tuple(plain_grads[k] for k in range(n_plain)) + (zero,) * n_tokens
+
+
+def ssm_in_batch_sum(users, items, ancs, poss, negs, temp: float, weights: InBatchWeights) -> torch.Tensor:
+    """The in-batch sampled softmax summed over the batch (formula in include/sslrec_b200.h, a28): for every pair
+    ln(sum_c w_c exp(s_bc)) - s_bb over the 2B columns [poss; negs], s_bc = cos(users[ancs[b]], items[id_c]) / temp,
+    w_c = weights.v[id_c] / B.  ``users`` / ``items`` as in ``ssm_loss_sum`` (a restricted view must mark every batch row);
+    under ``deterministic()`` every batch row's gradient is added in position order.  Reads and draws no candidates."""
+    dev = weights.v.device
+    ancs, poss, negs = _i64(ancs, dev), _i64(poss, dev), _i64(negs, dev)
+    B = ancs.numel()
+    if B < 1 or ancs.dim() != 1 or poss.shape != ancs.shape or negs.shape != ancs.shape:
+        raise RuntimeError('sslrec_b200: an in-batch softmax term needs B >= 1 pairs of one anchor, one positive and one negative')
+    if not 0.0 < C.c_float(temp).value < math.inf:
+        raise ValueError(f'sslrec_b200: the in-batch softmax temperature must be finite and > 0, got {temp!r}')
+    ops, plain = _mix_operands([users, items])
+    pack = (ops, ancs, poss, negs, float(temp), weights, len(plain))
+    return _SsmInBatchFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))
 
 
 # ---- HCCF's hyper-graph branch (hccf.py:43-49, HGNNLayer :100-108) on the library's skinny-GEMM kernels ---------------------
