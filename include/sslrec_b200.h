@@ -629,6 +629,16 @@ SSL_API int ssl_ssm_fwd_logq(const float *u_tbl, int64_t u_stride, const float *
  *   (every cosine low against popular, low-weight columns; at tau = 0.1 the offset alone is
  *   14.4) gets its loss and softmax weights at 2^-11: not fp32 grade.  The engine then takes
  *   3xTF32 (engine.contraction_kind, from the weight table's range, known on the host).
+ *   Every kernel forms a term as ex2(S - offset) * w_c, and ex2 is ex2.approx.ftz: a result below
+ *   2^-126 is 0.  S - offset = log2(e) (cos - 1) / tau >= -2 log2(e) / tau and w_c >= min v / B
+ *   (min over v > 0), so both ex2(S - offset) and the term are normal fp32 numbers when
+ *     2 log2(e) / tau + max(0, log2(B / min v)) <= 126.
+ *   Past it a row whose columns all sit near cos = -1 has rowsum 0 (loss -inf, colscale inf, then
+ *   NaN), and a row whose largest term is small loses its terms below the flush: its rowsum is
+ *   not fp32 grade.  engine.ssm_in_batch_sum refuses such a (B, tau, min v) with ValueError, on
+ *   the host, at 125 rather than 126: one binade for the rounding of S - offset, so a column
+ *   exactly opposite its row is not flushed by an ulp.  At B = 4096 and min v = 1 the smallest
+ *   tau is 0.0256; the sampled softmax's tau = 0.1 spans 40.9 binades.
  *   ssl_nce_bwd_cols: the column gradient.  For c < n (= 2B), in the fp32 order of
  *   csrc/ssm_in_batch.cuh:  d = (sum_s dt_part[s, c]) * colw[c];
  *     sink[ids[c]] += rinv_c (d - t^_c (t^_c . d))   (float atomics; ids NULL: row c, into a -0.0

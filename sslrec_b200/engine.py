@@ -1969,20 +1969,32 @@ def in_batch_weights(indptr, indices, n_item: int) -> np.ndarray:
 
 
 class InBatchWeights:
-    """``in_batch_weights`` on a device: ``v`` fp32 [n_item] (rounded once), and ``range``, max v / min v over the items with
-    v > 0, which bounds the weights of any batch's columns and picks the forward's kernel (``contraction_kind``) on the host."""
+    """``in_batch_weights`` on a device: ``v`` fp32 [n_item] (rounded once); ``range``, max v / min v over the items with
+    v > 0, which bounds the weights of any batch's columns and picks the forward's kernel (``contraction_kind``) on the host;
+    and ``vmin``, the smallest v > 0, which bounds the smallest term of the forward (``in_batch_binades``)."""
 
     def __init__(self, v, device):
         v32 = np.asarray(v).astype(np.float32)
         live = v32[v32 > 0].astype(np.float64)
         if v32.ndim != 1 or not np.all(np.isfinite(v32)) or live.size == 0 or (v32 < 0).any():
             raise ValueError('in-batch weights must be a finite, non-negative [n_item] vector with a positive entry')
-        self.n_item, self.range = int(v32.size), float(live.max() / live.min())
+        self.n_item, self.range, self.vmin = int(v32.size), float(live.max() / live.min()), float(live.min())
         self.v = torch.from_numpy(v32).to(device)
 
     @classmethod
     def of_matrix(cls, indptr, indices, n_item: int, device) -> 'InBatchWeights':
         return cls(in_batch_weights(indptr, indices, n_item), device)
+
+
+# the forward's terms w_c 2^(S - offset) stay normal fp32 numbers, which ex2.approx.ftz does not flush, while they span at most
+# this many binades below 1 (include/sslrec_b200.h, a28: 126, less one binade for the rounding of S - offset)
+IN_BATCH_MAX_BINADES = 125.0
+
+
+def in_batch_binades(B: int, temp: float, vmin: float) -> float:
+    """2 log2(e) / temp + max(0, log2(B / vmin)): how many binades below 1 the smallest term of the in-batch forward can lie
+    (a column opposite its row, the smallest weight vmin / B); the term is refused past IN_BATCH_MAX_BINADES."""
+    return 2.0 * LOG2E / float(temp) + max(0.0, math.log2(B / vmin))
 
 
 def _in_batch_rows(op) -> Rows:
@@ -2064,7 +2076,9 @@ def ssm_in_batch_sum(users, items, ancs, poss, negs, temp: float, weights: InBat
     """The in-batch sampled softmax summed over the batch (formula in include/sslrec_b200.h, a28): for every pair
     ln(sum_c w_c exp(s_bc)) - s_bb over the 2B columns [poss; negs], s_bc = cos(users[ancs[b]], items[id_c]) / temp,
     w_c = weights.v[id_c] / B.  ``users`` / ``items`` as in ``ssm_loss_sum`` (a restricted view must mark every batch row);
-    under ``deterministic()`` every batch row's gradient is added in position order.  Reads and draws no candidates."""
+    under ``deterministic()`` every batch row's gradient is added in position order.  Reads and draws no candidates.  Raises
+    ValueError when ``in_batch_binades(B, temp, weights.vmin)`` exceeds IN_BATCH_MAX_BINADES: a smaller term would be flushed
+    to 0 or lose digits (B, temp and vmin are host values, so CUDA-graph capture is unaffected)."""
     dev = weights.v.device
     ancs, poss, negs = _i64(ancs, dev), _i64(poss, dev), _i64(negs, dev)
     B = ancs.numel()
@@ -2072,6 +2086,11 @@ def ssm_in_batch_sum(users, items, ancs, poss, negs, temp: float, weights: InBat
         raise RuntimeError('sslrec_b200: an in-batch softmax term needs B >= 1 pairs of one anchor, one positive and one negative')
     if not 0.0 < C.c_float(temp).value < math.inf:
         raise ValueError(f'sslrec_b200: the in-batch softmax temperature must be finite and > 0, got {temp!r}')
+    binades = in_batch_binades(B, temp, weights.vmin)
+    if not binades <= IN_BATCH_MAX_BINADES:
+        raise ValueError(f'sslrec_b200: the in-batch softmax at tau {temp!r}, B {B} and smallest weight {weights.vmin:.6g} needs '
+                         f'2 log2(e) / tau + max(0, log2(B / min v)) <= {IN_BATCH_MAX_BINADES:g}, so that every term is a normal '
+                         f'fp32 number, got {binades:.4f}: raise tau or the smallest weight')
     ops, plain = _mix_operands([users, items])
     pack = (ops, ancs, poss, negs, float(temp), weights, len(plain))
     return _SsmInBatchFn.apply(pack, *plain, *_tokens(*[op for op in ops if isinstance(op, Rows)]))

@@ -290,6 +290,35 @@ def bpr_term_cases(ssm: bool):
     return out
 
 
+IN_BATCH_SMALLEST_TAU = 'min'      # the smallest tau engine.ssm_in_batch_sum accepts for the case's B and weights
+
+
+def in_batch_step_cases():
+    """(id, model_key, case name, hyper-parameter overrides, dim, tau, deterministic, tensor cores, the kernel the weighted
+    forward must take) of every whole step of train.ssm_in_batch: the goldens' ``small`` rows; each BPR model at every
+    BPR_TERM_DIMS at tau 0.1, on the train.deterministic route at d = 64 and at d = 64, tau 0.5 (3xFP16 on the graph of
+    ``path_case``); d = 32 at tau 0.1 and 0.5 for LightGCN and HCCF; NCL (3, 1) and LightGCL at IN_BATCH_SMALLEST_TAU; HCCF
+    on the FP32-FMA contraction."""
+    hccf = dict(hyper_num=128, keep_rate=0.5)
+    rows = [(f'{m}-small', m, 'small', {}, 64, BPR_TERM_TAU, False, True, 'tf32x3') for m in ('lightgcn', 'simgcl', 'sgl')]
+
+    def row(m, hp, d, tau, det=False, tc=True):
+        # tau 0.1: offset 14.4, past the weighted 3xFP16 bound; tau 0.5: 2.9 + (1 + log2 27.3) / 2 = 5.8 <= 13.5 on these graphs
+        kind = 'ffma' if not tc or d not in (32, 64) else 'f16x3' if tau == 0.5 else 'tf32x3'
+        rid = '-'.join([m] + [f'{k}{v}' for k, v in sorted(hp.items())]) + f'-paths-d{d}' + \
+            ('' if tau == BPR_TERM_TAU else f'-tau{tau}') + ('-det' if det else '') + ('' if tc else '-ffma')
+        return rid, m, 'paths', hp, d, tau, det, tc, kind
+
+    for m, hp in BPR_TERM_MODELS:
+        rows += [row(m, hp, d, BPR_TERM_TAU) for d in BPR_TERM_DIMS]
+        rows += [row(m, hp, 64, BPR_TERM_TAU, det=True), row(m, hp, 64, 0.5)]
+    for m, hp in (('lightgcn', {}), ('hccf', hccf)):
+        rows += [row(m, hp, 32, BPR_TERM_TAU), row(m, hp, 32, 0.5)]
+    rows += [row('ncl', dict(layer_num=3, high_order=1), 64, IN_BATCH_SMALLEST_TAU), row('lightgcl', dict(dropout=0), 64, IN_BATCH_SMALLEST_TAU)]
+    rows.append(row('hccf', hccf, 64, BPR_TERM_TAU, tc=False))
+    return rows
+
+
 def bpr_term_case_id(case):
     m, hp, d, M, tau = case
     return '-'.join([m] + [f'{k}{v}' for k, v in sorted(hp.items())] + [f'd{d}', f'M{M}'] + ([] if tau is None else [f'tau{tau}']))

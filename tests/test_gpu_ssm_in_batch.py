@@ -1,17 +1,20 @@
 """In-batch negatives for the sampled softmax (optional key train.ssm_in_batch) on the GPU.
 
 The term, through ``engine.ssm_in_batch_sum``: loss and the gradients into the user rows, the positive rows and every one of the
-2B columns against the float64 term of tests/inb_oracle.py, on each contraction kernel (FFMA at d = 48, 3xTF32, 3xFP16), at tau on
-both sides of 0.0902, B not a multiple of 64, duplicated ids among the columns, weights spanning four decades and cosines near
--1 as well as near 1; the kernel the forward took is the one ``contraction_kind`` names for the weights' range.  The FP32-FMA
-route (USE_TENSOR_CORES False) agrees with the tensor-core one.  Under train.deterministic the gradients are the staged
+2B columns against the float64 term of tests/inb_oracle.py, on each contraction kernel (FFMA at d = 20, 48 and 128, 3xTF32,
+3xFP16), at tau on both sides of 0.0902, B from 1 to 8192 (2B at and past a 64-column tile, B at and past a 128-row tile),
+duplicated ids among the columns, every column one item, zero weights, weights spanning four decades or scaled by 2^+-30, and
+cosines near -1 as well as near 1; the kernel the forward took is the one ``contraction_kind`` names for the weights' range.  The
+FP32-FMA route (USE_TENSOR_CORES False) agrees with the tensor-core one.  Under train.deterministic the gradients are the staged
 per-position contributions added in position order, bit for bit, and two runs are bit-identical.  ssl_nce_bwd_cols rejects bad
-arguments and writes nothing.
+arguments and writes nothing.  A temperature whose terms would fall below the flush of ex2.approx.ftz is refused; at the
+smallest accepted one a batch with every cosine <= -0.8 is within the float64 bounds.
 
 Models (LightGCN, SimGCL, SGL, NCL, HCCF, LightGCL): the key false is the key absent bit for bit; the step draws exactly the
-seeds of the plain step; under train.deterministic two runs and a CUDA-graph replay are bit-identical.  The whole step of
-LightGCN, SimGCL and SGL equals the float64 oracle with its BPR term replaced by the in-batch term.  SimGCL and NCL resumed from a
-mid-run checkpoint end bit-identical to an uninterrupted run."""
+seeds of the plain step; under train.deterministic two runs and a CUDA-graph replay are bit-identical.  The whole step of every
+BPR model equals the float64 oracle with its BPR term replaced by the in-batch term, on both gradient routes and each
+contraction kernel (ssl_test_helpers.in_batch_step_cases).  SimGCL and NCL resumed from a mid-run checkpoint end bit-identical
+to an uninterrupted run."""
 import numpy as np
 import pytest
 import torch
@@ -77,7 +80,30 @@ KERNEL_CASES = [  # (B, d, tau, weight range, anti-aligned rows, tensor cores, t
     (129, 32, 0.25, 1e2, False, True, 'f16x3'),
     (4096, 64, 0.2, 10.0, True, True, 'f16x3'),            # 7.2 + 2.2
     (1000, 64, 0.1, 1e4, True, False, 'ffma'),
+    (512, 128, 0.1, 1e4, True, True, 'ffma'),             # the lane layouts of ssl_nce_bwd_cols: 4 floats per lane, and
+    (300, 20, 0.1, 1e4, False, True, 'ffma'),             # 20 of 32 lanes idle
+    (8192, 64, 0.1, 1e4, False, True, 'tf32x3'),          # 16384 columns
+    (8192, 64, 0.5, 1e4, True, True, 'f16x3'),
 ]
+# one or two pairs; 2B at and past a 64-column tile (B = 32, 33); B at and past a 128-row tile (128, 129)
+KERNEL_CASES += [(B, 64, tau, 1e4, B in (33, 129), True, kind) for B in (1, 2, 32, 33, 128, 129)
+                 for tau, kind in ((0.1, 'tf32x3'), (0.5, 'f16x3'))]
+
+
+def _against_float64(loss, grads, users, items, ancs, poss, negs, tau, v32, v_loss=None):
+    """The bounds of ``test_term_against_float64`` against inb_oracle.term64 on the fp32 weights ``v32`` (float64 [n_item]);
+    ``v_loss``: another table whose float64 loss the loss must meet instead (the gradients keep the bound of ``v32``)."""
+    B = ancs.numel()
+    ref_leaves = [t.double().cuda().requires_grad_(True) for t in (users, items)]
+    ref = IB.term64(ref_leaves[0], ref_leaves[1], ancs, poss, negs, tau, v32)
+    ref.backward()
+    if v_loss is not None:
+        with torch.no_grad():
+            ref = IB.term64(users.double().cuda(), items.double().cuda(), ancs, poss, negs, tau, v_loss)
+    assert abs(loss - ref.item()) <= 1e-5 * max(1.0, abs(ref.item())) + 4e-7 * B / tau, (loss, ref.item())
+    A = IB.abs_scale(users.cuda(), items.cuda(), ancs, poss, negs, tau, v32)
+    for got, want, a, what in zip(grads, ref_leaves, A, ('users', 'items')):
+        H.close(got, want.grad, 2e-4, 5e-4 * a.cpu().numpy() + 1e-12, what)
 
 
 @pytest.mark.parametrize('B,d,tau,wrange,anti,tc,kind', KERNEL_CASES)
@@ -91,14 +117,7 @@ def test_term_against_float64(monkeypatch, B, d, tau, wrange, anti, tc, kind):
     loss, grads, took, w = _run(monkeypatch, users, items, ancs, poss, negs, v, tau)
     assert took == kind, (took, kind, w.range)
     assert w.range == pytest.approx(float(v.max() / v.min()), rel=1e-6)
-    v32 = w.v.double().cpu().numpy()
-    ref_leaves = [t.double().cuda().requires_grad_(True) for t in (users, items)]
-    ref = IB.term64(ref_leaves[0], ref_leaves[1], ancs, poss, negs, tau, v32)
-    ref.backward()
-    assert abs(loss - ref.item()) <= 1e-5 * max(1.0, abs(ref.item())) + 4e-7 * B / tau, (loss, ref.item())
-    A = IB.abs_scale(users.cuda(), items.cuda(), ancs, poss, negs, tau, v32)
-    for got, want, a, what in zip(grads, ref_leaves, A, ('users', 'items')):
-        H.close(got, want.grad, 2e-4, 5e-4 * a.cpu().numpy() + 1e-12, what)
+    _against_float64(loss, grads, users, items, ancs, poss, negs, tau, w.v.double().cpu().numpy())
     if anti:                                      # the rows do reach both ends of the cosine range
         u = torch.nn.functional.normalize(users[ancs].double(), dim=1)
         c = torch.nn.functional.normalize(items[torch.cat([poss, negs])].double(), dim=1)
@@ -125,9 +144,19 @@ def test_deterministic_route_is_its_ordered_restatement(monkeypatch):
     """Under train.deterministic the sinks receive the staged per-position contributions (users: ancs; items: the positives' row
     term at poss, then the 2B columns) added in position order: restated here with one torch add per position from the stages
     the route scattered.  A second run is bit-identical, and both are within the float64 bound."""
+    _ordered_restatement(monkeypatch, 300, 64)
+
+
+@pytest.mark.parametrize('B,d', [(1, 64), (200, 128)])
+def test_deterministic_route_is_its_ordered_restatement_at_one_pair_and_d128(monkeypatch, B, d):
+    """``test_deterministic_route_is_its_ordered_restatement`` at one pair (two columns) and at the widest row (FFMA)."""
+    _ordered_restatement(monkeypatch, B, d)
+
+
+def _ordered_restatement(monkeypatch, B, d):
     from sslrec_b200 import engine as E
     monkeypatch.setattr(E, 'DETERMINISTIC', True)
-    users, items, ancs, poss, negs, v = _case(300, 64, seed=3)
+    users, items, ancs, poss, negs, v = _case(B, d, seed=3)
     seen = []
     grouped = E._scatter_grouped
 
@@ -183,6 +212,76 @@ def test_bad_arguments_are_rejected_and_write_nothing():
     assert call(nn=0) == 0
     torch.cuda.synchronize()
     assert (sink == -7).all()
+
+
+@pytest.mark.parametrize('B,d,deterministic,kind', [(1000, 64, False, 'tf32x3'), (1000, 64, True, 'tf32x3'),
+                                                    (513, 128, False, 'ffma'), (513, 128, True, 'ffma')])
+def test_one_item_batch(monkeypatch, B, d, deterministic, kind):
+    """Every pair has the same anchor, positive and negative: all 2B columns are one item, so every column's gradient adds
+    into one row (the most contended atomic target), the 2B + B row terms into it under the ordered route."""
+    from sslrec_b200 import engine as E
+    monkeypatch.setattr(E, 'DETERMINISTIC', deterministic)
+    users, items, _, _, _, v = _case(B, d, seed=11)
+    ancs, poss, negs = torch.full((B,), 2), torch.full((B,), 7), torch.full((B,), 7)
+    loss, grads, took, w = _run(monkeypatch, users, items, ancs, poss, negs, v, 0.1)
+    assert took == kind
+    _against_float64(loss, grads, users, items, ancs, poss, negs, 0.1, w.v.double().cpu().numpy())
+    assert grads[1].abs().sum(1).nonzero().flatten().tolist() == [7] and grads[0].abs().sum(1).nonzero().flatten().tolist() == [2]
+
+
+@pytest.mark.parametrize('tau,kind', [(0.1, 'tf32x3'), (0.5, 'f16x3')])
+def test_zero_weights(monkeypatch, tau, kind):
+    """Weights of 0 at some of the batch's ids, pair 0's own positive among them: those columns add nothing to any row sum and
+    take no column gradient, while the pair's diagonal score still counts."""
+    from sslrec_b200 import engine as E
+    users, items, ancs, poss, negs, v = _case(400, 64, seed=12)
+    zero = [int(poss[0]), int(poss[3]), int(negs[1]), int(negs[10])]
+    v[zero] = 0.0
+    loss, grads, took, w = _run(monkeypatch, users, items, ancs, poss, negs, v, tau)
+    assert took == kind and w.vmin == float(np.float32(v[v > 0].min()))
+    _against_float64(loss, grads, users, items, ancs, poss, negs, tau, w.v.double().cpu().numpy())
+
+
+@pytest.mark.parametrize('tau,kind', [(0.1, 'tf32x3'), (0.5, 'f16x3')])
+@pytest.mark.parametrize('exponent', [30, -30])
+def test_absolute_weight_scale(monkeypatch, exponent, tau, kind):
+    """v times 2^30 or 2^-30 (exact in fp32): each loss_b moves by ln of the scale, the gradients do not.  The loss meets the
+    float64 loss of the scaled table, the gradients the bound of the unscaled one; the kernel is the unscaled table's."""
+    users, items, ancs, poss, negs, v = _case(600, 64, seed=13)
+    v32 = v.astype(np.float32).astype(np.float64)
+    scaled = v32 * 2.0 ** exponent
+    loss, grads, took, w = _run(monkeypatch, users, items, ancs, poss, negs, scaled, tau)
+    assert took == kind and np.array_equal(w.v.double().cpu().numpy(), scaled)
+    _against_float64(loss, grads, users, items, ancs, poss, negs, tau, v32, v_loss=scaled)
+
+
+@pytest.mark.parametrize('which', ['anti', 'partial'])
+def test_underflowing_temperature_is_refused(which):
+    """At tau = 0.02 the batches of inb_oracle.underflow_batch lose every term of a row ('anti': loss -inf) or a share of each
+    row sum far past fp32 grade ('partial') to the flush-to-zero ex2 (tests/test_host_ssm_in_batch.py restates it): the term
+    refuses the temperature, naming the bound, and so does the float just below the smallest accepted one."""
+    from sslrec_b200 import engine as E
+    users, items, ancs, poss, negs, v = IB.underflow_batch(which)
+    w = E.InBatchWeights(v, 'cuda')
+    tau = IB.smallest_tau(ancs.numel(), w.vmin)
+    for bad in (0.02, float(np.nextafter(tau, 0.0))):
+        leaves = [t.cuda().requires_grad_(True) for t in (users, items)]
+        with pytest.raises(ValueError, match=r'needs 2 log2\(e\) / tau \+ max\(0, log2\(B / min v\)\) <= 125'):
+            E.ssm_in_batch_sum(leaves[0], leaves[1], ancs.cuda(), poss.cuda(), negs.cuda(), bad, w)
+
+
+@pytest.mark.parametrize('tc,kind', [(False, 'ffma'), (True, 'tf32x3')])
+@pytest.mark.parametrize('which', ['anti', 'partial'])
+def test_smallest_accepted_temperature_is_within_float64(monkeypatch, which, tc, kind):
+    """The same batches at the smallest tau the bound accepts (~0.0247 for B = 300, min v ~ 1): every term is a normal fp32
+    number, and the loss and gradients meet the float64 bounds of ``test_term_against_float64``."""
+    from sslrec_b200 import engine as E
+    monkeypatch.setattr(E, 'USE_TENSOR_CORES', tc)
+    users, items, ancs, poss, negs, v = IB.underflow_batch(which)
+    tau = IB.smallest_tau(ancs.numel(), float(np.float32(v).min()))
+    loss, grads, took, w = _run(monkeypatch, users, items, ancs, poss, negs, v, tau)
+    assert took == kind and np.isfinite(loss)
+    _against_float64(loss, grads, users, items, ancs, poss, negs, tau, w.v.double().cpu().numpy())
 
 
 # ---- models ------------------------------------------------------------------------------------------------------------------
@@ -246,9 +345,10 @@ def test_two_runs_and_graph_replay_are_bit_identical(key):
             assert torch.equal(first[1][n_], other[1][n_]), (key, what, n_)
 
 
-def _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, tau):
+def _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, tau, tc=True):
     """One cal_loss + backward with the draws, k-means state and SVD factors injected (test_gpu_model_paths._gpu_model) and
-    train.ssm_in_batch; -> (dict(loss, parts, grads) of float64 numpy, the model, (case, hp, adj, draws, state))."""
+    train.ssm_in_batch; ``tau`` H.IN_BATCH_SMALLEST_TAU: the smallest the term accepts for the case's B and weights.  -> (dict(loss,
+    parts, grads) of float64 numpy, the model, (case, hp, adj, draws, state), tau, the kernels the contraction took)."""
     import sslrec_b200.config as cfgmod
     from oracle import cf_oracle as O
     from oracle import inputs, replay
@@ -261,6 +361,11 @@ def _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, 
         adj = O.normalized_adjacency(case['rows'], case['cols'], case['n_user'], case['n_item'])
         dr = replay.draws(model_key, case, hp, adj)
         st = H.path_state(model_key, case, hp, adj, dr)
+    margin = H.kink_margin(model_key, case, hp, adj, dr, st)
+    assert margin > H.KINK_MARGIN, f'ill-posed case: a kink input within {margin:.2e} of its |term| sum'
+    if tau == H.IN_BATCH_SMALLEST_TAU:
+        rowptr, cols = H.train_csr(case)
+        tau = IB.smallest_tau(len(case['ancs']), E.InBatchWeights.of_matrix(rowptr, cols, case['n_item'], 'cpu').vmin)
     default = cfgmod.default_config
 
     def with_train(name, **kw):
@@ -268,7 +373,18 @@ def _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, 
         cfg['train'].update(ssm_temperature=tau, ssm_in_batch=True, deterministic=deterministic)
         return cfg
 
+    kinds = []
+    kind = E.contraction_kind
+
+    def spy(*a, **k):                   # the weighted forward is the one caller that passes colscale_range
+        out = kind(*a, **k)
+        if k.get('colscale_range') is not None:
+            kinds.append(out)
+        return out
+
     monkeypatch.setattr(cfgmod, 'default_config', with_train)
+    monkeypatch.setattr(E, 'USE_TENSOR_CORES', tc)
+    monkeypatch.setattr(E, 'contraction_kind', spy)
     model = _gpu_model(model_key, case, hp, adj, dr, st)
     assert E.deterministic() == deterministic and model.ssm_in_batch
     model.zero_grad()
@@ -278,22 +394,23 @@ def _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, 
     monkeypatch.undo()
     got = dict(loss=loss.item(), parts={k: float(v) for k, v in parts.items()},
                grads={k: p.grad.double().cpu().numpy() for k, p in model.named_parameters()})
-    return got, model, (case, hp, adj, dr, st)
+    return got, model, (case, hp, adj, dr, st), tau, kinds
 
 
-WHOLE_STEP = [pytest.param(m, 'small', {}, 64, 0.1, False, id=f'{m}-small') for m in ('lightgcn', 'simgcl', 'sgl')]
-WHOLE_STEP += [pytest.param(m, 'paths', {}, d, 0.1, det, id=f'{m}-paths-d{d}' + ('-det' if det else ''))
-               for m in ('lightgcn', 'simgcl', 'sgl') for d, det in ((20, False), (64, False), (64, True), (128, False))]
-WHOLE_STEP += [pytest.param('lightgcn', 'paths', {}, 64, 0.5, False, id='lightgcn-paths-d64-tau0.5')]
+WHOLE_STEP = [pytest.param(*c[1:], id=c[0]) for c in H.in_batch_step_cases()]
+WORST = {}                              # (model, kernel) -> the largest error fraction of the whole-step rows run so far
 
 
-@pytest.mark.parametrize('model_key,case_name,hp_over,dim,tau,deterministic', WHOLE_STEP)
-def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, tau, deterministic):
+@pytest.mark.parametrize('model_key,case_name,hp_over,dim,tau,deterministic,tc,kind', WHOLE_STEP)
+def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, dim, tau, deterministic, tc, kind):
     """The step equals the float64 oracle with its BPR term replaced by inb_oracle.term64 on the loader's batch, with weights
-    from the case's training matrix (ssl_test_helpers.bpr_term_oracle): loss, every term and every gradient within the
-    path_errors bounds."""
+    from the case's training matrix (ssl_test_helpers.bpr_term_oracle): loss, every term and every parameter's gradient
+    (HCCF's hyper weights and LightGCL's Ws among them) within the path_errors bounds.  The weighted forward took ``kind``;
+    the weight table is in_batch_weights of the case's training CSR, bit for bit."""
     from sslrec_b200 import engine as E
-    got, model, (case, hp, adj, dr, st) = _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic, tau)
+    got, model, (case, hp, adj, dr, st), tau, kinds = _whole_step(monkeypatch, model_key, case_name, hp_over, dim, deterministic,
+                                                                  tau, tc)
+    assert kinds == [kind], (kinds, kind)
     assert 'bpr_loss' not in got['parts'] and model.dns_negs is None
     rowptr, cols = H.train_csr(case)
     v = E.in_batch_weights(rowptr, cols, case['n_item']).astype(np.float32)
@@ -303,8 +420,10 @@ def test_whole_step_against_float64(monkeypatch, model_key, case_name, hp_over, 
                             lambda u, i, _: IB.term64(u, i, ancs, poss, negs, tau, v.astype(np.float64)), 'ssm_loss')
     errs = H.path_errors(got, ref)
     worst = max(errs, key=errs.get)
-    print(f'in-batch {model_key}-{case_name}-d{dim}-tau{tau}{"-det" if deterministic else ""}: largest error '
-          f'{errs[worst]:.3f} of its bound ({worst})')
+    WORST[model_key, kind] = max(WORST.get((model_key, kind), 0.0), errs[worst])
+    print(f'in-batch {model_key}{hp_over}-{case_name}-d{dim}-tau{tau:.6g}{"-det" if deterministic else ""}-{kind}: largest '
+          f'error {errs[worst]:.3f} of its bound ({worst}); worst so far per (model, kernel): '
+          + ', '.join(f'{m}/{k} {e:.3f}' for (m, k), e in sorted(WORST.items())))
     assert errs[worst] <= 1.0, errs
 
 

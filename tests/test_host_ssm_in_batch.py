@@ -3,7 +3,10 @@ models and every refusal (no temperature, drawn candidates, popularity draws, Di
 gradient sync), the checkpoint record; ``engine.in_batch_weights`` against a brute-force float64 restatement of p_i and r_i;
 the loaders' sampling law itself (HostBatchLoader with ``sample_negs`` over many epochs: the column counts by a chi-square test,
 the weighted column sum as an unbiased estimate of the catalogue sum within a CLT bound); and the column-backward kernel
-(csrc/ssm_in_batch.cuh) under AddressSanitizer through tests/emu, bit for bit against its sequential float32 restatement."""
+(csrc/ssm_in_batch.cuh) under AddressSanitizer through tests/emu, bit for bit against its sequential float32 restatement.
+The forward's flush-to-zero terms restated in numpy (tests/inb_oracle.py): at tau = 0.02 they lose whole rows or fp32 grade,
+and ``engine.ssm_in_batch_sum`` refuses such a temperature.  On every whole-step case of tests/test_gpu_ssm_in_batch.py: the
+float32 oracle meets the GPU test's bounds against float64, and six wrong terms do not."""
 import os
 import shutil
 import subprocess
@@ -16,6 +19,8 @@ import scipy.sparse as sp
 import torch
 from scipy import stats
 
+import inb_oracle as IB
+import ssl_test_helpers as H
 from sslrec_b200 import engine as E
 from test_host_resume import make_run
 
@@ -240,3 +245,104 @@ def test_column_backward_matches_its_sequential_restatement_on_the_host(emulator
     r = subprocess.run([emulator] + [str(v) for v in case] + [str(sum(case) + 1)], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
     assert 'bad=0' in r.stdout
+
+
+# ---- the forward's flush-to-zero terms and the temperature bound -------------------------------------------------------------
+
+@pytest.mark.parametrize('which', ['anti', 'partial'])
+def test_flushed_terms_underflow_at_small_tau_and_the_bound_refuses_it(which):
+    """At tau = 0.02 the kernels' terms fp32(ex2.approx.ftz(S - offset)) w_c (inb_oracle.rowsum32) lose the batches of
+    inb_oracle.underflow_batch: every row sum of 'anti' is 0 (loss -inf), and each row sum of 'partial' misses far more than
+    fp32 grade.  ``engine.ssm_in_batch_sum`` refuses both before touching a device, with a message naming the bound, and so
+    does the next float below the smallest accepted tau; at that tau the same restatement is fp32 grade."""
+    users, items, ancs, poss, negs, v = IB.underflow_batch(which)
+    B = len(ancs)
+    cos = IB.cosines(users, items, ancs, poss, negs)
+    w = v.astype(np.float32)[np.concatenate([poss, negs])] / np.float32(B)
+    weights = E.InBatchWeights(v, 'cpu')
+    r32, r64 = IB.rowsum32(cos, w, 0.02), IB.rowsum64(cos, w, 0.02)
+    rel = np.abs(r32 / r64 - 1)
+    s_bb = cos[np.arange(B), np.arange(B)] / 0.02
+    with np.errstate(divide='ignore'):
+        loss = float(np.sum(np.log(r32) + 1 / 0.02 - s_bb))
+    print(f'{which} at tau 0.02: loss {loss}, row sums flushed to 0: {int((r32 == 0).sum())} of {B}, '
+          f'largest relative row-sum error {rel.max():.3g}')
+    if which == 'anti':
+        assert cos.max() <= -0.8 and (r32 == 0).all() and loss == -np.inf
+    else:
+        assert (r32 > 0).all() and rel.min() >= 1e-4
+    bound = r'needs 2 log2\(e\) / tau \+ max\(0, log2\(B / min v\)\) <= 125'
+    tau = IB.smallest_tau(B, weights.vmin)
+    for bad in (0.02, float(np.nextafter(tau, 0.0))):
+        with pytest.raises(ValueError, match=bound):
+            E.ssm_in_batch_sum(users, items, ancs, poss, negs, bad, weights)
+    assert 0.024 < tau < 0.025 and E.in_batch_binades(B, tau, weights.vmin) <= E.IN_BATCH_MAX_BINADES
+    rel = np.abs(IB.rowsum32(cos, w, tau) / IB.rowsum64(cos, w, tau) - 1)
+    assert rel.max() <= 1e-5, rel.max()
+
+
+def test_temperature_bound():
+    """in_batch_binades: 2 log2(e) / tau, plus log2(B / vmin) only when the smallest weight vmin / B is below 1 (a larger
+    weight cannot pull ex2's own result above the flush); ``vmin`` is the smallest positive weight after fp32 rounding."""
+    assert E.in_batch_binades(4096, 0.1, 1.0) == pytest.approx(2 * E.LOG2E / 0.1 + 12, rel=1e-15)
+    assert E.in_batch_binades(1, 0.1, 2.0 ** 30) == pytest.approx(2 * E.LOG2E / 0.1, rel=1e-15)
+    assert IB.smallest_tau(1, 2.0 ** 30) == IB.smallest_tau(1, 1.0)
+    assert 0.0255 < IB.smallest_tau(4096, 1.0) < 0.0256
+    w = E.InBatchWeights(np.array([0.0, 3.0, 1e-3 + 1e-12, 7.0]), 'cpu')
+    assert w.vmin == float(np.float32(1e-3 + 1e-12))
+    # every temperature of the existing in-batch cases is far inside the bound (B <= 8192, weights >= 2^-30)
+    assert E.in_batch_binades(8192, 0.05, 2.0 ** -30) < E.IN_BATCH_MAX_BINADES
+
+
+# ---- whole steps on host draws: the float32 oracle meets the bounds of tests/test_gpu_ssm_in_batch.py, wrong terms miss ----------
+
+def _step_cases():
+    seen, out = set(), []
+    for rid, m, name, hp, d, tau, _, _, _ in H.in_batch_step_cases():
+        if name == 'paths' and (m, repr(hp), d, tau) not in seen:
+            seen.add((m, repr(hp), d, tau))
+            out.append(pytest.param(m, hp, d, tau, id=rid))
+    return out
+
+
+def _popularity_only(case):
+    """The popularity-only law v = 1 / p_i (the negative slot's r_i dropped; a cold item clamped to p_i = 1 / |E|)."""
+    p = np.bincount(case['cols'], minlength=case['n_item']) / len(case['cols'])
+    return 1.0 / np.maximum(p, 1.0 / len(case['cols']))
+
+
+@pytest.mark.parametrize('model_key,hp_over,dim,tau', _step_cases())
+def test_whole_step_float32_meets_the_bounds_and_wrong_terms_do_not(model_key, hp_over, dim, tau):
+    """The float32 oracle is within path_errors of float64 on every whole-step case of the GPU test; each wrong term misses
+    them, by the reported factor: tau (1 + 1e-3), uniform weights, the popularity-only law, de-duplicated columns, the
+    columns ordered [negs; poss] (the diagonal read from the negatives).  w_c not divided by B shifts every loss_b by ln B
+    and leaves the gradients alone: its loss misses and its gradients pass."""
+    case, hp, adj, dr, st = H.bpr_term_setup(model_key, hp_over, dim)
+    assert H.kink_margin(model_key, case, hp, adj, dr, st) > H.KINK_MARGIN
+    ancs, poss, negs = (torch.from_numpy(case[k]) for k in ('ancs', 'poss', 'negs'))
+    rowptr, cols = H.train_csr(case)
+    v = E.in_batch_weights(rowptr, cols, case['n_item']).astype(np.float32).astype(np.float64)
+    if tau == H.IN_BATCH_SMALLEST_TAU:
+        tau = IB.smallest_tau(len(ancs), E.InBatchWeights(v, 'cpu').vmin)
+        assert 0.023 < tau < 0.025, tau
+
+    def run(dtype, t=tau, w=v, **kw):
+        return H.bpr_term_oracle(model_key, case, hp, adj, dr, st, dtype,
+                                 lambda u, i, _: IB.term64(u, i, ancs, poss, negs, t, w, **kw), 'ssm_loss')
+
+    ref = run(torch.float64)
+    ok = H.path_errors(run(torch.float32), ref)
+    assert max(ok.values()) <= 1.0, ok
+    wrong = {'tau (1 + 1e-3)': dict(t=tau * (1 + 1e-3)), 'uniform weights': dict(w=np.ones_like(v)),
+             'popularity-only weights': dict(w=_popularity_only(case)), 'de-duplicated columns': dict(dedup=True),
+             'columns [negs; poss]': dict(swap=True)}
+    report = [f'float32 {max(ok.values()):.3f}']
+    for what, kw in wrong.items():
+        bad = H.path_errors(run(torch.float32, **kw), ref)
+        assert max(bad.values()) > 1.0, (what, 'passes', bad)
+        report.append(f'{what} {max(bad.values()):.3g}')
+    bad = H.path_errors(run(torch.float32, per_b=False), ref)
+    grads = {k: e for k, e in bad.items() if k.startswith('grad_')}
+    assert bad['loss'] > 1.0 and bad['part_ssm_loss'] > 1.0 and max(grads.values()) <= 1.0, bad
+    report.append(f'w_c undivided: loss {bad["loss"]:.3g}, gradients {max(grads.values()):.3f}')
+    print('largest error as a fraction of its bound: ' + ', '.join(report))
